@@ -4,6 +4,7 @@
 
     python bench.py --gpus N --steps K --warmup W            (N>1: launched under torch.distributed.run)
     python bench.py --impl reference ...                     (CPU arm: the oracle port of the reference path)
+    python bench.py ... --dump-outputs DIR                   (also write the last timed step's outputs as DIR/<name>.npy)
 
 A "step" is ONE denoising step of the batch: one UNet evaluation at batch 16 (8 images x [uncond, cond])
 through the CUDA engine + the fused sampler update.  50 PLMS steps cost 51 UNet evaluations
@@ -63,11 +64,12 @@ def peaks():
         p = json.load(open(path))
         return dict(bf16_burst=p["bf16_tflops"], bf16_sustained=p["bf16_tflops_sustained"], hbm=p["hbm_gbs"],
                     source="MEASURED_PEAKS.json")
-    return dict(bf16_burst=1590.0, bf16_sustained=1400.0, hbm=6650.0, source="fallback (B200_PROFILING.md)")
+    return dict(bf16_burst=989.0, bf16_sustained=989.0, hbm=3350.0,
+                source="H100 SXM data sheet, dense, 700 W (not measured)")
 
 
 class ClockSampler:
-    """SM clock / throttle reasons DURING the timed region (B200_PROFILING.md recipe), sampled through NVML
+    """SM clock / throttle reasons DURING the timed region, sampled through NVML
     (same counters as the nvidia-smi query, but fast enough to get several samples inside a sub-second region)."""
 
     def __init__(self, index):
@@ -242,7 +244,7 @@ def gemm_roofline(prog, pk):
     achieved = tot_ops / (tot_ms * 1e-3) / 1e12
     peak = 2.0 * pk["bf16_sustained"]
     # DRAM bytes per GEMM launch (dram__bytes_read.sum + dram__bytes_write.sum, mean over one step's launches): from the
-    # ncu pass over this same command committed under profiles/ (tools/launch_summary.py --traffic), else null
+    # ncu pass over this same command stored under profiles/ (tools/launch_summary.py --traffic) when present, else null
     traffic, tsrc = None, None
     tf = os.path.join(ROOT, "profiles", f"r02_roofline_traffic_{WORKLOAD}.json")
     if os.path.exists(tf):
@@ -251,9 +253,9 @@ def gemm_roofline(prog, pk):
         traffic, tsrc = tj.get("gemm_dram_bytes_per_launch"), tj.get("source")
     return dict(bound="tensor", achieved=achieved, peak=peak, unit="TOP/s", frac=achieved / peak, traffic=traffic,
                 traffic_source=tsrc,
-                kernel="gemm_i8_kernel (tcgen05.mma kind::i8)", launches=len(evs), gemm_ms_per_step=tot_ms,
+                kernel="gemm_i8_kernel (wgmma m64nNk32 s32.u8/s8.s8)", launches=len(evs), gemm_ms_per_step=tot_ms,
                 algorithmic_ops_per_step=tot_ops,
-                peak_source=f"2 x bf16_tflops_sustained ({pk['source']}); INT8 dense = 2x bf16 on sm_100a",
+                peak_source=f"2 x bf16_tflops_sustained ({pk['source']}); INT8 dense = 2x bf16 on sm_90a",
                 note="events bracket each launch individually (serialised, includes launch gaps)")
 
 
@@ -269,6 +271,9 @@ def main():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-roofline", action="store_true")
     ap.add_argument("--no-graph", action="store_true", help="launch kernels individually (for ncu launch lists)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last timed step returned (x_prev, eps) as DIR/<name>.npy "
+                         "(float32); the same arguments give the same inputs, so two builds can be compared output for output")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3) if args.impl == "b200" else args.warmup
     if args.impl == "reference":
@@ -343,6 +348,7 @@ def main():
     ctx = c_host.to(dev) if c_host is not None else None
     nxt = torch.empty_like(x)
     e_t = torch.empty_like(x)
+    torch.manual_seed(44)                        # the sampler's eps history and eta > 0 noise: same draws in every run
     old = [torch.randn_like(x) for _ in range(3)]
 
     def step(i, x_in, nxt, ctx_dev):
@@ -358,6 +364,7 @@ def main():
         noise = torch.randn_like(x_in) if sigma[k] != 0.0 else None
         samplers._step(x_in, eps, nxt, a_t=a_t, a_prev=a_prev, sigma=sigma[k], cfg_scale=CFG_SCALE, coef=coef,
                        olds=tuple(old[:olds_n]) + (None,) * (3 - olds_n), eps_out=e_t if olds_n else None, noise=noise)
+        return eps
 
     def barrier():
         if dist is not None:
@@ -372,11 +379,14 @@ def main():
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         torch.cuda.profiler.start()    # no-op unless run under `ncu --profile-from-start off` (profiles/: launch list)
         e0.record()
+        eps_last = None
         for i in range(args.steps):
-            step(args.warmup + i, x, nxt, ctx)
+            eps_last = step(args.warmup + i, x, nxt, ctx)
         e1.record()
         barrier()
         torch.cuda.profiler.stop()
+    # outputs of the last timed step, taken before the e2e loop below reuses the buffers
+    dumps = {"x_prev": nxt.float().cpu(), "eps": eps_last.float().cpu()} if args.dump_outputs and eps_last is not None else None
     ms = e0.elapsed_time(e1)
     launches = L.qd_launch_count() - launches0
     prog = qnn.program(x, ctx, cfg_dedup=True) if cfg_dedup else qnn.program(torch.cat([x, x]) if guided else x, ctx)
@@ -434,7 +444,7 @@ def main():
         "config": {"workload": w["desc"],
                    "step": f"1 denoising step = 1 UNet evaluation at batch {UB} + fused sampler update",
                    "unet_step_ms": ms_step, "unet_evals_per_image_batch": UNET_EVALS_PER_IMAGE_BATCH,
-                   "l2": "working set per step (int8 weights + GBs of activations) is far larger than the 126 MB L2",
+                   "l2": "working set per step (int8 weights + GBs of activations) is far larger than the 50 MB L2",
                    "cfg_prefix_dedup": bool(cfg_dedup),
                    "cfg_note": ("the guided batch [x; x] shares its UNet prefix up to the first cross-attention; the engine runs that "
                                 "prefix once (bit-identical eps); whole_step_int8_tops counts the FULL batch-16 evaluation, "
@@ -458,6 +468,12 @@ def main():
         torch.set_num_threads(host_threads())
         cb = cpu_baseline(ckpt)
         line["cpu_baseline"] = cb
+    if dumps is not None:
+        import numpy as np
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        for name, t in dumps.items():
+            np.save(os.path.join(args.dump_outputs, f"{name}.npy"), t.numpy().astype(np.float32))
+        line["dumped_outputs"] = {name: list(t.shape) for name, t in dumps.items()}
     print(json.dumps(line))
     if dist is not None:
         dist.destroy_process_group()

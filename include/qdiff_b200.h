@@ -1,5 +1,5 @@
 /*
- * qdiff_b200 -- C ABI of the B200-native quantized-diffusion UNet engine (libqdiff_b200.so).
+ * qdiff_b200 -- C ABI of the H100-native (sm_90a) quantized-diffusion UNet engine (libqdiff_b200.so).
  *
  * The reference (Xiuyu-Li/q-diffusion) has no FFI layer: its boundary is the Python class API of
  * `qdiff` (QuantModel.forward, qdiff/quant_model.py:68-69) and every op underneath is a PyTorch
@@ -39,7 +39,7 @@ typedef struct qd_qparams {
 
 /* ------------------------------------------------------------------------------------------
  * qd_qgemm_i8 -- QuantModule.forward (qdiff/quant_layer.py:248-279) for Conv2d 3x3 (stride 1,
- * pad 1), Conv2d 1x1, Conv1d k=1 and Linear, as INT8 tcgen05 GEMM with the de-quantisation fused
+ * pad 1), Conv2d 1x1, Conv1d k=1 and Linear, as INT8 wgmma GEMM with the de-quantisation fused
  * into the epilogue:
  *   y[m,n] = scale[n] * (sum_k a[m,k] * w[n,k] - corr[cls(m)][n]) + bias[n]
  *            (+ rowvec[m / rows_per_batch][n]) (+ residual[m,n])
@@ -110,13 +110,13 @@ typedef struct qd_gemm_desc {
    * a_bf16 = 1: `a` holds the activation as THREE bfloat16 planes per pixel, [M][3][Cp] (hi, mid, lo with
    * x = hi + mid + lo to 2^-24 relative, written by qd_split_bf16x3), `w` the zero-point-free weight codes as bfloat16
    * [n_rows][taps][3][Cp] (the codes repeated for the three planes: |code| <= 255 is exact in bfloat16), C = BYTES per
-   * tap = 6 * Cp, lda in bytes.  The contraction runs on tcgen05.mma kind::f16 with fp32 accumulation, so
+   * tap = 6 * Cp, lda in bytes.  The contraction runs on wgmma bf16 x bf16 with fp32 accumulation, so
    * y = scale[n] * sum_k x[m,k] * ws[n,k] + bias (+ rowvec, + residual) carries fp32-level rounding only
    * (qdiff/quant_layer.py:263-279 with use_act_quant False).  No corr, no out_q, no geglu. */
   int32_t a_bf16;
   /* out_q_f16 = 1 (row-major out_q only): out_q receives fp16 values (code - zero_point) instead of 8-bit codes; ldq and
-   * out_q_head_pitch then count fp16 elements.  Operand format of qd_attention_desc.qk_f16 (the attention's QK^T on
-   * tcgen05.mma kind::f16: the same integers, no zero-point correction pass).  The centred code is an integer of
+   * out_q_head_pitch then count fp16 elements.  Operand format of qd_attention_desc.qk_f16 (the attention's QK^T
+   * on f16 MMAs: the same integers, no zero-point correction pass).  The centred code is an integer of
    * magnitude <= 255, exact in fp16. */
   int32_t out_q_f16;
 } qd_gemm_desc;
@@ -300,9 +300,9 @@ typedef struct qd_attention_desc {
   void* out_q;           /* optional: codes of the consumer's activation quantizer `oq` (to_out / proj_out input) */
   long long ld_out_q;
   qd_qparams oq;
-  /* qk_f16 = 1: q and k hold fp16 values (code - zero_point) in the per-head padded layout (head_stride_q = head_stride_k
-   * = 128 BYTES, d <= 64; ld_q / ld_k / offsets in bytes as always); zq / zk / q_signed / k_signed / ws are ignored.
-   * Same result as the code path (exact integer arithmetic in fp32); tcgen05 kernel only. */
+  /* qk_f16 = 1: q and k hold fp16 values (code - zero_point) in the per-head padded layout (head_stride_q, head_stride_k
+   * >= 2 d BYTES, d <= 64; ld_q / ld_k / offsets in bytes as always); zq / zk / q_signed / k_signed / ws are ignored.
+   * Same result as the code path (exact integer arithmetic in fp32); d in {16, 24, 32, 40, 48, 64}. */
   int32_t qk_f16;
   int32_t reserved5;
 } qd_attention_desc;

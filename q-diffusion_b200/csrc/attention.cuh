@@ -17,7 +17,7 @@
 //   * K / V^T tiles stream through a cp.async double buffer, one __syncthreads per tile
 //   * 8 warps x 16 query rows per CTA; the key permutation lets the S accumulator fragment feed the PV
 //     A-operand without shuffles: MMA k-slot (4t+e) <-> key 8*(e>>1)+2t+(e&1) inside each 32-key chunk.
-// Tensor path: legacy mma.sync IMMA (register-resident P); see DESIGN.md for why tcgen05 does not pay here yet.
+// Tensor path: mma.sync IMMA (register-resident P).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -50,6 +50,13 @@ __device__ __forceinline__ void mma_i8_16832(int (&c)[4], const uint32_t (&a)[4]
 __device__ __forceinline__ void cp_async8(void* smem_dst, const void* gsrc) {
   asm volatile("cp.async.ca.shared.global [%0], [%1], 8;" ::"r"((uint32_t)__cvta_generic_to_shared(smem_dst)), "l"(gsrc) : "memory");
 }
+// fp16 operands, fp32 accumulation (qd_attention_desc.qk_f16).  With the fragments loaded exactly like the 8-bit ones
+// (8 bytes per lane and 32-byte chunk), the k-slots see the same consistent permutation of the head dim in A and B.
+__device__ __forceinline__ void mma_f16_16816(float (&c)[4], const uint32_t (&a)[4], const uint32_t (&b)[2]) {
+  asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.f16.f16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
+               : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3])
+               : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b[0]), "r"(b[1]));
+}
 __device__ __forceinline__ void cp_async16(void* smem_dst, const void* gsrc) {
   asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"((uint32_t)__cvta_generic_to_shared(smem_dst)), "l"(gsrc) : "memory");
 }
@@ -70,8 +77,8 @@ __host__ __device__ __forceinline__ int att_vt_perm(int t) {
 }
 
 // zq * rowsum_d(k[b, j, head h]) for every key: the only zero-point cross term that survives the softmax.
-// bias_minus = 0: ws = zq*rowsum (subtracted by the mma.sync kernel).  Otherwise ws = bias - zq*rowsum, ADDED to the raw
-// score by the tcgen05 kernel: with bias = 0x4B400000 the sum is at once the corrected score and its magic-number float form.
+// bias_minus = 0: ws = zq*rowsum (subtracted by the mma.sync kernel).  Otherwise ws = bias - zq*rowsum, to be ADDED to the
+// raw score: with bias = 0x4B400000 the sum is at once the corrected score and its magic-number float form.
 template <bool SIGNED>
 __global__ void att_krowsum_kernel(const qd_attention_desc p, int tk_pad, int bias_minus = 0, int bias = 0) {
   const long long total = (long long)p.B * p.heads * tk_pad;
@@ -126,12 +133,15 @@ __device__ __forceinline__ float att_i2f(int s) {
 }
 
 // DQ: reduction length of QK^T padded to a multiple of 32; DV: head dim d (multiple of 8).
-// v2.1 (profiles/r01_attention_v2.txt): shared-memory tiles are addressed from the array symbol (the
-// pointer-array version compiled to generic LD + 64-bit IMAD address math, 30% of all instructions), the
+// Shared-memory tiles are addressed from the array symbol (the
+// pointer-array version compiled to generic LD + 64-bit IMAD address math), the
 // int<->float conversions avoid the XU pipe (it was the binding unit: I2F + F2I + 2 MUFU per score at
 // 16 lanes/clk/SM), and the d index inside a 32-byte k-chunk is permuted (slot 4t+e <-> d 8t+e, slot
 // 16+4t+e <-> d 8t+4+e, identically for Q and K) so each B fragment is one 8-byte shared load.
-template <int DQ, int DV, bool QK_SIGNED, bool V_SIGNED, bool SM16, int MINB>
+// F16: Q / K hold fp16 centred codes (code - zero point; qd_attention_desc.qk_f16, d <= 64).  QK^T then runs as
+// m16n8k16 f16 x f16 -> f32: every product and partial sum is an integer below 2^24, so the score is exact, and it is
+// already free of zero-point cross terms (no zq*rowsum(k) pass).  DQ counts BYTES of the padded reduction in both forms.
+template <int DQ, int DV, bool QK_SIGNED, bool V_SIGNED, bool SM16, int MINB, bool F16 = false>
 __global__ void __launch_bounds__(ATT_WARPS * 32, MINB)
 qattention_kernel(const qd_attention_desc p) {
   constexpr int KP = att_kp(DQ);    // K tile row pitch (bytes): odd multiple of 32 -> conflict-free 8-byte B-fragment loads
@@ -141,7 +151,9 @@ qattention_kernel(const qd_attention_desc p) {
   constexpr int KB = ATT_BN * KP, VB = (DV + 8) * VP;
   constexpr int ZB = ATT_BN * 4;    // per-tile zq*rowsum(k) slice
   constexpr bool MAGIC = DV <= 64;  // |S| <= 255*255*d < 2^22
-  constexpr int WPR = DV / 8;       // 8-byte pieces per K row
+  constexpr int RB = F16 ? 2 * DV : DV;   // bytes of one head's Q / K row
+  constexpr int WPR = RB / 8;       // 8-byte pieces per K row
+  static_assert(!F16 || DV <= 64, "fp16 Q / K operands: d <= 64 keeps |S| below 2^22");
   extern __shared__ __align__(16) uint8_t att_smem[];
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -173,7 +185,7 @@ qattention_kernel(const qd_attention_desc p) {
       const int r = idx / WPR, w = idx - r * WPR;
       cp_async8(dK + r * KP + 8 * w, kbase + (long long)(j0 + r) * p.ld_k + 8 * w);
     }
-    if (p.zq != 0 && threadIdx.x < ATT_BN / 4)
+    if (!F16 && p.zq != 0 && threadIdx.x < ATT_BN / 4)
       cp_async16(att_smem + 2 * KB + 2 * VB + buf * ZB + 16 * threadIdx.x, zrk_g + j0 + 4 * threadIdx.x);
     if (pass == 1) {
       uint8_t* dV = att_smem + 2 * KB + buf * VB;
@@ -197,15 +209,15 @@ qattention_kernel(const qd_attention_desc p) {
 #pragma unroll
     for (int kc = 0; kc < NKC; ++kc) {
       const int c0 = kc * 32 + 8 * t, c1 = c0 + 4;
-      qf[kc][0] = c0 < DV ? *reinterpret_cast<const uint32_t*>(q0 + c0) : 0u;
-      qf[kc][1] = c0 < DV ? *reinterpret_cast<const uint32_t*>(q1 + c0) : 0u;
-      qf[kc][2] = c1 < DV ? *reinterpret_cast<const uint32_t*>(q0 + c1) : 0u;
-      qf[kc][3] = c1 < DV ? *reinterpret_cast<const uint32_t*>(q1 + c1) : 0u;
+      qf[kc][0] = c0 < RB ? *reinterpret_cast<const uint32_t*>(q0 + c0) : 0u;
+      qf[kc][1] = c0 < RB ? *reinterpret_cast<const uint32_t*>(q1 + c0) : 0u;
+      qf[kc][2] = c1 < RB ? *reinterpret_cast<const uint32_t*>(q0 + c1) : 0u;
+      qf[kc][3] = c1 < RB ? *reinterpret_cast<const uint32_t*>(q1 + c1) : 0u;
     }
   }
   // s2 = S_int * c  with c = sim_scale * log2(e)
   const float c = p.sim_scale * 1.4426950408889634f;
-  const bool has_zq = p.zq != 0;
+  const bool has_zq = !F16 && p.zq != 0;
   const bool ragged = (p.Tk % ATT_BN) != 0;
 
   int mi0 = INT_MIN, mi1 = INT_MIN;   // running integer row maxima (of S_raw - zrk)
@@ -245,11 +257,17 @@ qattention_kernel(const qd_attention_desc p) {
 #pragma unroll
       for (int nt = 0; nt < 8; ++nt) {
         sacc[nt][0] = sacc[nt][1] = sacc[nt][2] = sacc[nt][3] = 0;
+        [[maybe_unused]] float facc[4] = {0.f, 0.f, 0.f, 0.f};
 #pragma unroll
         for (int kc = 0; kc < NKC; ++kc) {
           const uint2 kk = *reinterpret_cast<const uint2*>(sK + (8 * nt + g) * KP + kc * 32 + 8 * t);
           const uint32_t bf[2] = {kk.x, kk.y};
-          mma_i8_16832<QK_SIGNED, QK_SIGNED>(sacc[nt], qf[kc], bf);
+          if constexpr (F16) mma_f16_16816(facc, qf[kc], bf);
+          else mma_i8_16832<QK_SIGNED, QK_SIGNED>(sacc[nt], qf[kc], bf);
+        }
+        if constexpr (F16) {     // exact integers in fp32
+          sacc[nt][0] = __float2int_rn(facc[0]); sacc[nt][1] = __float2int_rn(facc[1]);
+          sacc[nt][2] = __float2int_rn(facc[2]); sacc[nt][3] = __float2int_rn(facc[3]);
         }
       }
       if (has_zq) {
@@ -370,8 +388,8 @@ qattention_kernel(const qd_attention_desc p) {
 //   * K, V^T and zq*rowsum(k) are staged in shared memory ONCE per CTA (the row sums are computed here: no
 //     separate att_krowsum launch) and each warp then streams 16-query slabs past them;
 //   * the softmax is a single pass over register-resident scores (max, sum, codes from the same accumulators).
-// The two-pass kernels above pay their per-CTA prologue (tile ring, barriers, TMEM allocation for the tcgen05
-// one) per 128 queries; with ~80 keys that prologue was 90% of the run time (profiles/r01_cross_attention.txt).
+// The two-pass kernel above pays its per-CTA prologue (tile ring, barriers) per 128 queries; with ~80 keys that
+// prologue dominates the run time.
 // Arithmetic is the same as qattention_kernel (same exp2-domain formulas, same fragment/key permutations).
 constexpr int ATS_WARPS = 4;
 

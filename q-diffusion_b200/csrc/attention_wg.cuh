@@ -1,0 +1,464 @@
+// Quantised attention on sm_90a warpgroup MMAs: qattention_kernel's two-pass algorithm (integer scores, exp2-domain
+// softmax with the calibrated step, P codes as hi/lo byte planes, integer PV, row sums from an all-ones V^T row) with
+//   * S = Q K^T as wgmma m64n64 (k32 on 8-bit codes, or k16 f16 x f16 -> f32 on fp16 centred codes - qk_f16 - whose
+//     integer scores are exact), Q fragments in registers, the K tile in shared memory;
+//   * O += P V as wgmma m64nNV k32 (u8 P codes in registers, V^T tile in shared memory), NV = d + 8 rounded up to a
+//     wgmma width (the extra rows: the all-ones row, then zeros);
+//   * K, V^T and the zq*rowsum(k) slice staged by TMA / bulk copies through an ATW_STAGES-deep mbarrier ring (one load
+//     per (pass, key tile); pass 0 needs no V^T).
+// Two consumer warpgroups, 64 query rows each.  The per-warp accumulator fragment of wgmma m64nN is the m16n8 fragment
+// of mma.sync repeated over N / 8 column tiles, and the register A operand has the m16n8k32 layout, so the softmax code
+// below is qattention_kernel's, operating on the same registers.  V^T keeps its 16-key byte permutation
+// (att_vt_perm): with it, the P fragments built from the S accumulators are the A operand without shuffles.
+#pragma once
+#include "attention.cuh"
+#include "ptx.cuh"
+
+namespace qd {
+
+__device__ __forceinline__ void wgmma_ra_s8s8_n64(uint32_t* d, const uint32_t (&a)[4], uint64_t db, uint32_t scale_d) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t"
+      "setp.ne.b32 p, %37, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k32.s32.s8.s8 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, {%32, %33, %34, %35}, %36, p;\n\t}\n"
+      : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]), "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15]), "+r"(d[16]), "+r"(d[17]), "+r"(d[18]), "+r"(d[19]), "+r"(d[20]), "+r"(d[21]), "+r"(d[22]), "+r"(d[23]), "+r"(d[24]), "+r"(d[25]), "+r"(d[26]), "+r"(d[27]), "+r"(d[28]), "+r"(d[29]), "+r"(d[30]), "+r"(d[31])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(scale_d));
+}
+__device__ __forceinline__ void wgmma_ra_u8u8_n64(uint32_t* d, const uint32_t (&a)[4], uint64_t db, uint32_t scale_d) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t"
+      "setp.ne.b32 p, %37, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k32.s32.u8.u8 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, {%32, %33, %34, %35}, %36, p;\n\t}\n"
+      : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]), "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15]), "+r"(d[16]), "+r"(d[17]), "+r"(d[18]), "+r"(d[19]), "+r"(d[20]), "+r"(d[21]), "+r"(d[22]), "+r"(d[23]), "+r"(d[24]), "+r"(d[25]), "+r"(d[26]), "+r"(d[27]), "+r"(d[28]), "+r"(d[29]), "+r"(d[30]), "+r"(d[31])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(scale_d));
+}
+__device__ __forceinline__ void wgmma_ra_f16_n64(float* d, const uint32_t (&a)[4], uint64_t db, uint32_t scale_d) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t"
+      "setp.ne.b32 p, %37, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, {%32, %33, %34, %35}, %36, p, 1, 1, 0;\n\t}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(scale_d));
+}
+__device__ __forceinline__ void wgmma_ra_u8u8_n24(uint32_t* d, const uint32_t (&a)[4], uint64_t db, uint32_t scale_d) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t"
+      "setp.ne.b32 p, %17, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n24k32.s32.u8.u8 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11}, {%12, %13, %14, %15}, %16, p;\n\t}\n"
+      : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]), "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(scale_d));
+}
+__device__ __forceinline__ void wgmma_ra_u8s8_n24(uint32_t* d, const uint32_t (&a)[4], uint64_t db, uint32_t scale_d) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t"
+      "setp.ne.b32 p, %17, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n24k32.s32.u8.s8 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11}, {%12, %13, %14, %15}, %16, p;\n\t}\n"
+      : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]), "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(scale_d));
+}
+__device__ __forceinline__ void wgmma_ra_u8u8_n32(uint32_t* d, const uint32_t (&a)[4], uint64_t db, uint32_t scale_d) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t"
+      "setp.ne.b32 p, %21, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n32k32.s32.u8.u8 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, {%16, %17, %18, %19}, %20, p;\n\t}\n"
+      : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]), "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(scale_d));
+}
+__device__ __forceinline__ void wgmma_ra_u8s8_n32(uint32_t* d, const uint32_t (&a)[4], uint64_t db, uint32_t scale_d) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t"
+      "setp.ne.b32 p, %21, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n32k32.s32.u8.s8 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, {%16, %17, %18, %19}, %20, p;\n\t}\n"
+      : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]), "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(scale_d));
+}
+__device__ __forceinline__ void wgmma_ra_u8u8_n48(uint32_t* d, const uint32_t (&a)[4], uint64_t db, uint32_t scale_d) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t"
+      "setp.ne.b32 p, %29, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n48k32.s32.u8.u8 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23}, {%24, %25, %26, %27}, %28, p;\n\t}\n"
+      : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]), "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15]), "+r"(d[16]), "+r"(d[17]), "+r"(d[18]), "+r"(d[19]), "+r"(d[20]), "+r"(d[21]), "+r"(d[22]), "+r"(d[23])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(scale_d));
+}
+__device__ __forceinline__ void wgmma_ra_u8s8_n48(uint32_t* d, const uint32_t (&a)[4], uint64_t db, uint32_t scale_d) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t"
+      "setp.ne.b32 p, %29, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n48k32.s32.u8.s8 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23}, {%24, %25, %26, %27}, %28, p;\n\t}\n"
+      : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]), "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15]), "+r"(d[16]), "+r"(d[17]), "+r"(d[18]), "+r"(d[19]), "+r"(d[20]), "+r"(d[21]), "+r"(d[22]), "+r"(d[23])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(scale_d));
+}
+__device__ __forceinline__ void wgmma_ra_u8s8_n64(uint32_t* d, const uint32_t (&a)[4], uint64_t db, uint32_t scale_d) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t"
+      "setp.ne.b32 p, %37, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k32.s32.u8.s8 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, {%32, %33, %34, %35}, %36, p;\n\t}\n"
+      : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]), "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15]), "+r"(d[16]), "+r"(d[17]), "+r"(d[18]), "+r"(d[19]), "+r"(d[20]), "+r"(d[21]), "+r"(d[22]), "+r"(d[23]), "+r"(d[24]), "+r"(d[25]), "+r"(d[26]), "+r"(d[27]), "+r"(d[28]), "+r"(d[29]), "+r"(d[30]), "+r"(d[31])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(scale_d));
+}
+__device__ __forceinline__ void wgmma_ra_u8u8_n80(uint32_t* d, const uint32_t (&a)[4], uint64_t db, uint32_t scale_d) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t"
+      "setp.ne.b32 p, %45, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n80k32.s32.u8.u8 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39}, {%40, %41, %42, %43}, %44, p;\n\t}\n"
+      : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]), "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15]), "+r"(d[16]), "+r"(d[17]), "+r"(d[18]), "+r"(d[19]), "+r"(d[20]), "+r"(d[21]), "+r"(d[22]), "+r"(d[23]), "+r"(d[24]), "+r"(d[25]), "+r"(d[26]), "+r"(d[27]), "+r"(d[28]), "+r"(d[29]), "+r"(d[30]), "+r"(d[31]), "+r"(d[32]), "+r"(d[33]), "+r"(d[34]), "+r"(d[35]), "+r"(d[36]), "+r"(d[37]), "+r"(d[38]), "+r"(d[39])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(scale_d));
+}
+__device__ __forceinline__ void wgmma_ra_u8s8_n80(uint32_t* d, const uint32_t (&a)[4], uint64_t db, uint32_t scale_d) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t"
+      "setp.ne.b32 p, %45, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n80k32.s32.u8.s8 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39}, {%40, %41, %42, %43}, %44, p;\n\t}\n"
+      : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]), "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15]), "+r"(d[16]), "+r"(d[17]), "+r"(d[18]), "+r"(d[19]), "+r"(d[20]), "+r"(d[21]), "+r"(d[22]), "+r"(d[23]), "+r"(d[24]), "+r"(d[25]), "+r"(d[26]), "+r"(d[27]), "+r"(d[28]), "+r"(d[29]), "+r"(d[30]), "+r"(d[31]), "+r"(d[32]), "+r"(d[33]), "+r"(d[34]), "+r"(d[35]), "+r"(d[36]), "+r"(d[37]), "+r"(d[38]), "+r"(d[39])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(scale_d));
+}
+__device__ __forceinline__ void wgmma_ra_u8u8_n96(uint32_t* d, const uint32_t (&a)[4], uint64_t db, uint32_t scale_d) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t"
+      "setp.ne.b32 p, %53, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n96k32.s32.u8.u8 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47}, {%48, %49, %50, %51}, %52, p;\n\t}\n"
+      : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]), "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15]), "+r"(d[16]), "+r"(d[17]), "+r"(d[18]), "+r"(d[19]), "+r"(d[20]), "+r"(d[21]), "+r"(d[22]), "+r"(d[23]), "+r"(d[24]), "+r"(d[25]), "+r"(d[26]), "+r"(d[27]), "+r"(d[28]), "+r"(d[29]), "+r"(d[30]), "+r"(d[31]), "+r"(d[32]), "+r"(d[33]), "+r"(d[34]), "+r"(d[35]), "+r"(d[36]), "+r"(d[37]), "+r"(d[38]), "+r"(d[39]), "+r"(d[40]), "+r"(d[41]), "+r"(d[42]), "+r"(d[43]), "+r"(d[44]), "+r"(d[45]), "+r"(d[46]), "+r"(d[47])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(scale_d));
+}
+__device__ __forceinline__ void wgmma_ra_u8s8_n96(uint32_t* d, const uint32_t (&a)[4], uint64_t db, uint32_t scale_d) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t"
+      "setp.ne.b32 p, %53, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n96k32.s32.u8.s8 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47}, {%48, %49, %50, %51}, %52, p;\n\t}\n"
+      : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]), "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15]), "+r"(d[16]), "+r"(d[17]), "+r"(d[18]), "+r"(d[19]), "+r"(d[20]), "+r"(d[21]), "+r"(d[22]), "+r"(d[23]), "+r"(d[24]), "+r"(d[25]), "+r"(d[26]), "+r"(d[27]), "+r"(d[28]), "+r"(d[29]), "+r"(d[30]), "+r"(d[31]), "+r"(d[32]), "+r"(d[33]), "+r"(d[34]), "+r"(d[35]), "+r"(d[36]), "+r"(d[37]), "+r"(d[38]), "+r"(d[39]), "+r"(d[40]), "+r"(d[41]), "+r"(d[42]), "+r"(d[43]), "+r"(d[44]), "+r"(d[45]), "+r"(d[46]), "+r"(d[47])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(scale_d));
+}
+__device__ __forceinline__ void wgmma_ra_u8u8_n112(uint32_t* d, const uint32_t (&a)[4], uint64_t db, uint32_t scale_d) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t"
+      "setp.ne.b32 p, %61, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n112k32.s32.u8.u8 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55}, {%56, %57, %58, %59}, %60, p;\n\t}\n"
+      : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]), "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15]), "+r"(d[16]), "+r"(d[17]), "+r"(d[18]), "+r"(d[19]), "+r"(d[20]), "+r"(d[21]), "+r"(d[22]), "+r"(d[23]), "+r"(d[24]), "+r"(d[25]), "+r"(d[26]), "+r"(d[27]), "+r"(d[28]), "+r"(d[29]), "+r"(d[30]), "+r"(d[31]), "+r"(d[32]), "+r"(d[33]), "+r"(d[34]), "+r"(d[35]), "+r"(d[36]), "+r"(d[37]), "+r"(d[38]), "+r"(d[39]), "+r"(d[40]), "+r"(d[41]), "+r"(d[42]), "+r"(d[43]), "+r"(d[44]), "+r"(d[45]), "+r"(d[46]), "+r"(d[47]), "+r"(d[48]), "+r"(d[49]), "+r"(d[50]), "+r"(d[51]), "+r"(d[52]), "+r"(d[53]), "+r"(d[54]), "+r"(d[55])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(scale_d));
+}
+__device__ __forceinline__ void wgmma_ra_u8s8_n112(uint32_t* d, const uint32_t (&a)[4], uint64_t db, uint32_t scale_d) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t"
+      "setp.ne.b32 p, %61, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n112k32.s32.u8.s8 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55}, {%56, %57, %58, %59}, %60, p;\n\t}\n"
+      : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]), "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15]), "+r"(d[16]), "+r"(d[17]), "+r"(d[18]), "+r"(d[19]), "+r"(d[20]), "+r"(d[21]), "+r"(d[22]), "+r"(d[23]), "+r"(d[24]), "+r"(d[25]), "+r"(d[26]), "+r"(d[27]), "+r"(d[28]), "+r"(d[29]), "+r"(d[30]), "+r"(d[31]), "+r"(d[32]), "+r"(d[33]), "+r"(d[34]), "+r"(d[35]), "+r"(d[36]), "+r"(d[37]), "+r"(d[38]), "+r"(d[39]), "+r"(d[40]), "+r"(d[41]), "+r"(d[42]), "+r"(d[43]), "+r"(d[44]), "+r"(d[45]), "+r"(d[46]), "+r"(d[47]), "+r"(d[48]), "+r"(d[49]), "+r"(d[50]), "+r"(d[51]), "+r"(d[52]), "+r"(d[53]), "+r"(d[54]), "+r"(d[55])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(scale_d));
+}
+
+constexpr int ATW_STAGES = 3;
+constexpr int ATW_THREADS = ATT_WARPS * 32;       // two warpgroups
+// PV width: d + 8 (the all-ones row sits at row d) rounded up to a wgmma N for 8-bit operands
+__host__ __device__ constexpr int atw_nv(int DV) {
+  return DV + 8 <= 24 ? 24 : DV + 8 <= 32 ? 32 : DV + 8 <= 48 ? 48 : DV + 8 <= 64 ? 64 : DV + 8 <= 80 ? 80 : DV + 8 <= 96 ? 96 : 112;
+}
+struct AtwSmem {
+  int k_bytes, v_bytes, z_off, bar_off, total;
+};
+// per stage: K tile 64 x P bytes (P-byte swizzle), V^T tile NV x 64 bytes (64-byte swizzle), 256 bytes of row sums
+__host__ __device__ inline AtwSmem atw_smem(int P, int NV) {
+  AtwSmem l;
+  l.k_bytes = (ATT_BN * P + 1023) / 1024 * 1024;
+  l.v_bytes = (NV * ATT_BN + 1023) / 1024 * 1024;
+  l.z_off = ATW_STAGES * (l.k_bytes + l.v_bytes);
+  l.bar_off = l.z_off + ATW_STAGES * ATT_BN * 4;
+  l.total = l.bar_off + 2 * ATW_STAGES * 8 + 1024;   // + alignment slack
+  return l;
+}
+// sm_90 shared-memory descriptor for a K-major tile of `row_bytes`-byte rows stored with the matching TMA swizzle
+__device__ __forceinline__ uint64_t atw_desc(uint32_t addr, int row_bytes) {
+  const uint64_t layout = row_bytes == 128 ? 1 : row_bytes == 64 ? 2 : 3;
+  uint64_t d = (uint64_t)((addr & 0x3FFFF) >> 4);
+  d |= (uint64_t)1 << 16;
+  d |= (uint64_t)((8 * row_bytes) >> 4) << 32;
+  d |= layout << 62;
+  return d;
+}
+
+template <int N, bool VS>
+__device__ __forceinline__ void atw_pv(uint32_t* d, const uint32_t (&a)[4], uint64_t db) {
+  if constexpr (VS) {
+    if constexpr (N == 24) wgmma_ra_u8s8_n24(d, a, db, 1u);
+    else if constexpr (N == 32) wgmma_ra_u8s8_n32(d, a, db, 1u);
+    else if constexpr (N == 48) wgmma_ra_u8s8_n48(d, a, db, 1u);
+    else if constexpr (N == 64) wgmma_ra_u8s8_n64(d, a, db, 1u);
+    else if constexpr (N == 80) wgmma_ra_u8s8_n80(d, a, db, 1u);
+    else if constexpr (N == 96) wgmma_ra_u8s8_n96(d, a, db, 1u);
+    else wgmma_ra_u8s8_n112(d, a, db, 1u);
+  } else {
+    if constexpr (N == 24) wgmma_ra_u8u8_n24(d, a, db, 1u);
+    else if constexpr (N == 32) wgmma_ra_u8u8_n32(d, a, db, 1u);
+    else if constexpr (N == 48) wgmma_ra_u8u8_n48(d, a, db, 1u);
+    else if constexpr (N == 64) wgmma_ra_u8u8_n64(d, a, db, 1u);
+    else if constexpr (N == 80) wgmma_ra_u8u8_n80(d, a, db, 1u);
+    else if constexpr (N == 96) wgmma_ra_u8u8_n96(d, a, db, 1u);
+    else wgmma_ra_u8u8_n112(d, a, db, 1u);
+  }
+}
+
+// DQ: bytes of the padded QK^T reduction (multiple of 32, <= P); DV: head dim d; P: per-head pitch of Q / K in bytes
+// (32 / 64 / 128, also the K tile's swizzle span).
+template <int DQ, int DV, bool QK_SIGNED, bool V_SIGNED, bool SM16, bool F16>
+__global__ void __launch_bounds__(ATW_THREADS, 1)
+qattention_wg_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_constant__ CUtensorMap tmV,
+                     const qd_attention_desc p, int P) {
+  constexpr int NV = atw_nv(DV);
+  constexpr int NKC = DQ / 32;      // 32-byte k-steps of QK^T
+  constexpr int NDT = DV / 8 + 1;   // n8 tiles of the output + the row-sum tile
+  constexpr bool MAGIC = DV <= 64;  // |S| <= 255*255*d < 2^22
+  constexpr int RB = F16 ? 2 * DV : DV;   // bytes of one head's Q / K row
+  static_assert(!F16 || DV <= 64, "fp16 Q / K operands: d <= 64 keeps |S| below 2^22");
+  extern __shared__ uint8_t atw_raw[];
+  uint8_t* smem = atw_raw + (((smem_u32(atw_raw) + 1023u) & ~1023u) - smem_u32(atw_raw));
+  const AtwSmem lay = atw_smem(P, NV);
+  uint64_t* full = reinterpret_cast<uint64_t*>(smem + lay.bar_off);
+  uint64_t* empty = full + ATW_STAGES;
+
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int g = lane >> 2, t = lane & 3;
+  const int bh = blockIdx.y;
+  const int b = bh / p.heads, h = bh - b * p.heads;
+  const int row0 = blockIdx.x * ATT_BM + warp * 16;
+  const int ntiles = (p.Tk + ATT_BN - 1) / ATT_BN;
+  const int nloads = 2 * ntiles;      // (pass, tile) in order
+  const bool has_zq = !F16 && p.zq != 0;
+  const int* zrk_g = reinterpret_cast<const int*>(p.ws) + (long long)bh * (long long)att_ws_stride(p.Tk);
+
+  // ---- V^T rows d .. NV-1 of every stage: the all-ones row, then zeros (TMA writes rows 0 .. d-1 only).  A row of
+  // equal bytes is the same under any swizzle.
+  for (int i = threadIdx.x; i < ATW_STAGES * (NV - DV) * ATT_BN; i += ATW_THREADS) {
+    const int s = i / ((NV - DV) * ATT_BN), r = (i / ATT_BN) % (NV - DV) + DV, c = i % ATT_BN;
+    smem[ATW_STAGES * lay.k_bytes + s * lay.v_bytes + r * ATT_BN + c] = r == DV ? 1 : 0;
+  }
+  if (threadIdx.x == 0) {
+    tma_prefetch_desc(&tmK);
+    tma_prefetch_desc(&tmV);
+    for (int s = 0; s < ATW_STAGES; ++s) {
+      mbar_init(&full[s], 1);
+      mbar_init(&empty[s], ATT_WARPS);
+    }
+    fence_mbar_init();
+  }
+  fence_proxy_async();     // the generic writes above -> visible to the tensor cores
+  __syncthreads();
+
+  auto issue = [&](int L) {           // thread 0: load number L into stage L % ATW_STAGES
+    const int s = L % ATW_STAGES, pass = L / ntiles, tile = L - pass * ntiles;
+    const int j0 = tile * ATT_BN;
+    const uint32_t bytes = (uint32_t)(ATT_BN * P) + (pass ? (uint32_t)(ATT_BN * DV) : 0u) + (has_zq ? ATT_BN * 4u : 0u);
+    mbar_arrive_expect_tx(&full[s], bytes);
+    tma_load_2d(smem + s * lay.k_bytes, &tmK, &full[s], h * P, b * p.Tk + j0);
+    if (pass) tma_load_2d(smem + ATW_STAGES * lay.k_bytes + s * lay.v_bytes, &tmV, &full[s], j0, bh * DV);
+    if (has_zq) bulk_load_1d(smem + lay.z_off + s * ATT_BN * 4, zrk_g + j0, ATT_BN * 4, &full[s]);
+  };
+  if (threadIdx.x == 0)
+    for (int L = 0; L < ATW_STAGES && L < nloads; ++L) issue(L);
+
+  // ---- Q fragments (rows g, g+8 of this warp's 16-row slab) in the m16n8k32 / m16n8k16 A layout: bytes 4t.. and
+  // 16+4t.. of every 32-byte k-chunk; zero beyond the head's row (the K tile may hold the next head's bytes there).
+  uint32_t qf[NKC][4];
+  {
+    const uint8_t* qbase = reinterpret_cast<const uint8_t*>(p.q) + (long long)b * p.Tq * p.ld_q + p.q_off + h * p.head_stride_q;
+    const int r0 = min(row0 + g, p.Tq - 1), r1 = min(row0 + g + 8, p.Tq - 1);
+    const uint8_t* q0 = qbase + (long long)r0 * p.ld_q;
+    const uint8_t* q1 = qbase + (long long)r1 * p.ld_q;
+#pragma unroll
+    for (int kc = 0; kc < NKC; ++kc) {
+      const int c0 = kc * 32 + 4 * t, c1 = c0 + 16;
+      qf[kc][0] = c0 < RB ? *reinterpret_cast<const uint32_t*>(q0 + c0) : 0u;
+      qf[kc][1] = c0 < RB ? *reinterpret_cast<const uint32_t*>(q1 + c0) : 0u;
+      qf[kc][2] = c1 < RB ? *reinterpret_cast<const uint32_t*>(q0 + c1) : 0u;
+      qf[kc][3] = c1 < RB ? *reinterpret_cast<const uint32_t*>(q1 + c1) : 0u;
+    }
+  }
+  const float c = p.sim_scale * 1.4426950408889634f;
+  const bool ragged = (p.Tk % ATT_BN) != 0;
+  int mi0 = INT_MIN, mi1 = INT_MIN;
+  float l0 = 0.f, l1 = 0.f;
+  float off0 = 0.f, off1 = 0.f;
+  uint32_t olo[NV / 2], ohi[SM16 ? NV / 2 : 1];
+#pragma unroll
+  for (int i = 0; i < NV / 2; ++i) olo[i] = 0u;
+#pragma unroll
+  for (int i = 0; i < (SM16 ? NV / 2 : 1); ++i) ohi[i] = 0u;
+  const float pmax = (float)p.p_qmax;
+  const QuantK oqk = make_quantk(p.oq);
+
+  for (int pass = 0; pass < 2; ++pass) {
+    if (pass == 1) {
+      l0 += __shfl_xor_sync(0xffffffffu, l0, 1);
+      l0 += __shfl_xor_sync(0xffffffffu, l0, 2);
+      l1 += __shfl_xor_sync(0xffffffffu, l1, 1);
+      l1 += __shfl_xor_sync(0xffffffffu, l1, 2);
+      off0 = -(float)mi0 * c + log2f(1.0f / (l0 * p.delta_w));
+      off1 = -(float)mi1 * c + log2f(1.0f / (l1 * p.delta_w));
+    }
+    for (int tile = 0; tile < ntiles; ++tile) {
+      const int L = pass * ntiles + tile, st = L % ATW_STAGES;
+      const uint32_t ph = (uint32_t)(L / ATW_STAGES) & 1u;
+      const int j0 = tile * ATT_BN;
+      mbar_wait(&full[st], ph);
+      const uint64_t dK = atw_desc(smem_u32(smem + st * lay.k_bytes), P);
+      const int* sZrk = reinterpret_cast<const int*>(smem + lay.z_off + st * ATT_BN * 4);
+
+      // ---- S = Q K^T for this warpgroup: 64 x 64; this warp's 16 rows land in sacc[nt][*] (m16n8 fragments)
+      int sacc[8][4];
+      {
+        uint32_t si[32];
+        float sf[F16 ? 32 : 1];
+        wgmma_fence();
+#pragma unroll
+        for (int kc = 0; kc < NKC; ++kc) {
+          if constexpr (F16) wgmma_ra_f16_n64(sf, qf[kc], dK + (uint64_t)(2 * kc), kc ? 1u : 0u);
+          else if constexpr (QK_SIGNED) wgmma_ra_s8s8_n64(si, qf[kc], dK + (uint64_t)(2 * kc), kc ? 1u : 0u);
+          else wgmma_ra_u8u8_n64(si, qf[kc], dK + (uint64_t)(2 * kc), kc ? 1u : 0u);
+        }
+        wgmma_commit();
+        wgmma_wait<0>();
+        if constexpr (F16) {
+#pragma unroll
+          for (int i = 0; i < 32; ++i) asm volatile("" : "+f"(sf[i])::"memory");
+#pragma unroll
+          for (int i = 0; i < 32; ++i) sacc[i >> 2][i & 3] = __float2int_rn(sf[i]);     // exact integers
+        } else {
+#pragma unroll
+          for (int i = 0; i < 32; ++i) asm volatile("" : "+r"(si[i])::"memory");
+#pragma unroll
+          for (int i = 0; i < 32; ++i) sacc[i >> 2][i & 3] = (int)si[i];
+        }
+      }
+      if (has_zq) {
+#pragma unroll
+        for (int nt = 0; nt < 8; ++nt) {
+          const int2 z = *reinterpret_cast<const int2*>(sZrk + 8 * nt + 2 * t);
+          sacc[nt][0] -= z.x; sacc[nt][1] -= z.y; sacc[nt][2] -= z.x; sacc[nt][3] -= z.y;
+        }
+      }
+      if (ragged && tile == ntiles - 1) {
+#pragma unroll
+        for (int nt = 0; nt < 8; ++nt) {
+          const int j = j0 + 8 * nt + 2 * t;
+          if (j >= p.Tk) { sacc[nt][0] = -(1 << 21); sacc[nt][2] = -(1 << 21); }
+          if (j + 1 >= p.Tk) { sacc[nt][1] = -(1 << 21); sacc[nt][3] = -(1 << 21); }
+        }
+      }
+      if (pass == 0) {
+        int tm0 = sacc[0][0], tm1 = sacc[0][2];
+#pragma unroll
+        for (int nt = 0; nt < 8; ++nt) {
+          tm0 = max(tm0, max(sacc[nt][0], sacc[nt][1]));
+          tm1 = max(tm1, max(sacc[nt][2], sacc[nt][3]));
+        }
+        tm0 = max(tm0, __shfl_xor_sync(0xffffffffu, tm0, 1));
+        tm0 = max(tm0, __shfl_xor_sync(0xffffffffu, tm0, 2));
+        tm1 = max(tm1, __shfl_xor_sync(0xffffffffu, tm1, 1));
+        tm1 = max(tm1, __shfl_xor_sync(0xffffffffu, tm1, 2));
+        if (tm0 > mi0) { l0 *= (mi0 == INT_MIN) ? 0.f : ex2_approx((float)(mi0 - tm0) * c); mi0 = tm0; }
+        if (tm1 > mi1) { l1 *= (mi1 == INT_MIN) ? 0.f : ex2_approx((float)(mi1 - tm1) * c); mi1 = tm1; }
+        const float b0 = -(float)mi0 * c, b1 = -(float)mi1 * c;
+        float a0 = 0.f, a1 = 0.f;
+#pragma unroll
+        for (int nt = 0; nt < 8; ++nt) {
+          a0 += ex2_approx(fmaf(att_i2f<MAGIC>(sacc[nt][0]), c, b0)) + ex2_approx(fmaf(att_i2f<MAGIC>(sacc[nt][1]), c, b0));
+          a1 += ex2_approx(fmaf(att_i2f<MAGIC>(sacc[nt][2]), c, b1)) + ex2_approx(fmaf(att_i2f<MAGIC>(sacc[nt][3]), c, b1));
+        }
+        l0 += a0;
+        l1 += a1;
+      } else {
+        // ---- P codes packed straight into A fragments (byte planes), then O += P V on the warpgroup
+        const uint64_t dV = atw_desc(smem_u32(smem + ATW_STAGES * lay.k_bytes + st * lay.v_bytes), ATT_BN);
+        uint32_t plo[2][4], phi[2][4];
+#pragma unroll
+        for (int kc = 0; kc < 2; ++kc) {
+#pragma unroll
+          for (int half = 0; half < 2; ++half) {
+            const int ntA = 4 * kc + 2 * half, ntB = ntA + 1;
+            uint32_t cd[8];
+            const int sv[8] = {sacc[ntA][0], sacc[ntA][1], sacc[ntB][0], sacc[ntB][1],
+                               sacc[ntA][2], sacc[ntA][3], sacc[ntB][2], sacc[ntB][3]};
+#pragma unroll
+            for (int e = 0; e < 8; ++e) {
+              const float pr = ex2_approx(fmaf(att_i2f<MAGIC>(sv[e]), c, e < 4 ? off0 : off1));
+              cd[e] = __float_as_uint(fminf(pr, pmax) + 12582912.0f);
+            }
+            plo[kc][2 * half] = __byte_perm(__byte_perm(cd[0], cd[1], 0x0040), __byte_perm(cd[2], cd[3], 0x0040), 0x5410);
+            plo[kc][2 * half + 1] = __byte_perm(__byte_perm(cd[4], cd[5], 0x0040), __byte_perm(cd[6], cd[7], 0x0040), 0x5410);
+            if constexpr (SM16) {
+              phi[kc][2 * half] = __byte_perm(__byte_perm(cd[0], cd[1], 0x0051), __byte_perm(cd[2], cd[3], 0x0051), 0x5410);
+              phi[kc][2 * half + 1] = __byte_perm(__byte_perm(cd[4], cd[5], 0x0051), __byte_perm(cd[6], cd[7], 0x0051), 0x5410);
+            }
+          }
+        }
+        wgmma_fence();
+#pragma unroll
+        for (int kc = 0; kc < 2; ++kc) {
+          atw_pv<NV, V_SIGNED>(olo, plo[kc], dV + (uint64_t)(2 * kc));
+          if constexpr (SM16) atw_pv<NV, V_SIGNED>(ohi, phi[kc], dV + (uint64_t)(2 * kc));
+        }
+        wgmma_commit();
+        wgmma_wait<0>();
+#pragma unroll
+        for (int i = 0; i < NV / 2; ++i) asm volatile("" : "+r"(olo[i])::"memory");
+#pragma unroll
+        for (int i = 0; i < (SM16 ? NV / 2 : 1); ++i) asm volatile("" : "+r"(ohi[i])::"memory");
+      }
+      // ---- this warp is done with the stage; thread 0 refills it once every warp is
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&empty[st]);
+      if (threadIdx.x == 0 && L + ATW_STAGES < nloads) {
+        mbar_wait(&empty[st], ph);
+        issue(L + ATW_STAGES);
+      }
+      __syncwarp();
+    }
+  }
+
+  // ---- write O: (256*hi + lo - zv * rowsum) * out_scale.  Row sums: column d (tile NDT - 1, t == 0).
+  float rs0 = (float)(int)olo[4 * (NDT - 1)], rs1 = (float)(int)olo[4 * (NDT - 1) + 2];
+  if constexpr (SM16) { rs0 += 256.0f * (float)(int)ohi[4 * (NDT - 1)]; rs1 += 256.0f * (float)(int)ohi[4 * (NDT - 1) + 2]; }
+  rs0 = __shfl_sync(0xffffffffu, rs0, lane & ~3);
+  rs1 = __shfl_sync(0xffffffffu, rs1, lane & ~3);
+  const int r0 = row0 + g, r1 = row0 + g + 8;
+  const float z0 = (float)p.zv * rs0, z1 = (float)p.zv * rs1;
+#pragma unroll
+  for (int nd = 0; nd < NDT - 1; ++nd) {
+    const int col = h * DV + 8 * nd + 2 * t;
+    float v0 = (float)(int)olo[4 * nd], v1 = (float)(int)olo[4 * nd + 1], v2 = (float)(int)olo[4 * nd + 2], v3 = (float)(int)olo[4 * nd + 3];
+    if constexpr (SM16) {
+      v0 += 256.0f * (float)(int)ohi[4 * nd]; v1 += 256.0f * (float)(int)ohi[4 * nd + 1];
+      v2 += 256.0f * (float)(int)ohi[4 * nd + 2]; v3 += 256.0f * (float)(int)ohi[4 * nd + 3];
+    }
+    const float y0 = (v0 - z0) * p.out_scale, y1 = (v1 - z0) * p.out_scale;
+    const float y2 = (v2 - z1) * p.out_scale, y3 = (v3 - z1) * p.out_scale;
+    if (p.out) {
+      if (r0 < p.Tq) *reinterpret_cast<float2*>(p.out + ((long long)b * p.Tq + r0) * p.ld_out + col) = make_float2(y0, y1);
+      if (r1 < p.Tq) *reinterpret_cast<float2*>(p.out + ((long long)b * p.Tq + r1) * p.ld_out + col) = make_float2(y2, y3);
+    }
+    if (p.out_q) {
+      uint8_t* oq = reinterpret_cast<uint8_t*>(p.out_q);
+      if (r0 < p.Tq)
+        *reinterpret_cast<uint16_t*>(oq + ((long long)b * p.Tq + r0) * p.ld_out_q + col) =
+            (uint16_t)(quant_code(y0, oqk) | (quant_code(y1, oqk) << 8));
+      if (r1 < p.Tq)
+        *reinterpret_cast<uint16_t*>(oq + ((long long)b * p.Tq + r1) * p.ld_out_q + col) =
+            (uint16_t)(quant_code(y2, oqk) | (quant_code(y3, oqk) << 8));
+    }
+  }
+}
+
+}  // namespace qd

@@ -289,7 +289,7 @@ __global__ void __launch_bounds__(256) attention_fp32_rows_kernel(const qd_atten
 // Three-kernel path (large feature maps).  Pass 1: a block reduces `slab` pixels x all channels to per-GROUP
 // partial sums (fp32 per thread over the slab, then double, in a fixed order: results are run-to-run
 // identical).  The slab length is chosen by the launcher so that the grid fills the GPU at every level of the
-// UNet (the fixed 64-pixel slabs left the 8x8 / 16x16 levels with 16-64 blocks: 40 us for 5 MB).
+// UNet (fixed 64-pixel slabs would leave the 8x8 / 16x16 levels with only 16-64 blocks).
 // ws layout: double part[B][nslab][groups][2], then float stats[B][groups][2].
 constexpr int GN_MAX_GROUPS = 64;
 __global__ void __launch_bounds__(256) gn_partial_kernel(const float* __restrict__ x, long long ld_x, int HW, int C,
@@ -350,8 +350,7 @@ __global__ void __launch_bounds__(256) gn_finalize_kernel(const double* __restri
 // Statistics from the producing GEMMs' epilogues (qd_gemm_desc.gn_stats): per 32-row slab and channel (sum, sum of squares).
 // One block per (group, image): 128 threads stride over the group's (slab, channel) items, accumulate in double, reduce
 // in a fixed order (warp shuffles, then the 4 warps through shared memory).  Replaces gn_partial + gn_finalize, i.e. one
-// full read of the fp32 tensor (SD: 2.5 GB per step, profiles/r01_launches_step_final.summary.txt).  (The first version
-// used one block per IMAGE: 16 blocks walking 330 KB each were slower than the pass they replaced.)
+// full read of the fp32 tensor.  (One block per IMAGE instead leaves most SMs idle.)
 __global__ void __launch_bounds__(128) gn_finalize_from_stats_kernel(const float2* __restrict__ slabs, long long ld_stats,
                                                                     int HW, int C, int groups, float eps,
                                                                     float* __restrict__ stats) {
@@ -392,11 +391,10 @@ __global__ void __launch_bounds__(128) gn_finalize_from_stats_kernel(const float
 // quad: it folds mean / rstd / gamma / beta (/ scale-shift) into y = a*x + b once (8 registers) and then streams its rows,
 // GN_BATCH independent 16-byte loads in flight before the first store.  The first version (one block of C/4 threads per
 // 32 rows, up to 4 quads per thread) needed 118 registers and ran 96-thread blocks at 21 % occupancy: every warp sat
-// on its first FFMA waiting for DRAM (profiles/r02_gn_apply_before.txt: 1.8-3 TB/s).  The consumer count and the raw
+// on its first FFMA waiting for DRAM.  The consumer count and the raw
 // output are template parameters so that the common single-consumer case carries one quantizer's constants only.
-// Occupancy (round 2, profiles/r02_gn_apply_variants.txt): the single-consumer kernel waited on DRAM with 24 of 64 warps
-// resident (79 registers, 8-row load batches).  4-row batches under a 64-register cap (4 blocks = 32 warps per SM) are 6-10 %
-// faster on every UNet's shapes; 6 blocks per SM spill and lose 30 %.  The multi-consumer / raw-output variants keep 8 rows.
+// Occupancy: the single-consumer kernel runs 4-row load batches under a 64-register cap (4 blocks = 32 warps per SM) so
+// that more warps wait on DRAM at once; the multi-consumer / raw-output variants keep 8 rows.
 constexpr int GN_BATCH = 8;                                   // host: rows per block are multiples of GN_BATCH * TY
 __host__ __device__ constexpr int gn_apply_batch(int NOUT, bool RAW) { return (NOUT <= 1 && !RAW) ? 4 : 8; }
 __host__ __device__ constexpr int gn_apply_minblocks(int NOUT, bool RAW) { return (NOUT <= 1 && !RAW) ? 4 : 1; }
@@ -564,7 +562,7 @@ __global__ void __launch_bounds__(512) gn_fused_small_kernel(const qd_groupnorm_
 
 // ------------------------------------------------------------------------------------ layernorm
 // One warp per row; the row lives in registers (NVEC float4 per lane, compile-time so it is NOT demoted to local
-// memory: the first version indexed a float4[32] array with a run-time trip count and spilled it, profiles/r01_*),
+// memory: the first version indexed a float4[32] array with a run-time trip count and spilled it),
 // two-pass mean / variance in fp32, then 1-3 consumer quantizers.
 template <int NVEC>
 __global__ void __launch_bounds__(256) layernorm_quant_kernel(const qd_layernorm_desc p) {

@@ -15,7 +15,7 @@
 
 #include "../../include/qdiff_b200.h"
 #include "attention.cuh"
-#include "attention_tc.cuh"
+#include "attention_wg.cuh"
 #include "elem.cuh"
 #include "gemm_i8.cuh"
 
@@ -43,8 +43,8 @@ int check_launch(const char* what) {
 
 // Every kernel launch of the library goes through here.
 // Programmatic dependent launch (cudaLaunchAttributeProgrammaticStreamSerialization on every launch + griddepcontrol.wait /
-// launch_dependents in every kernel) was built and MEASURED in round 2: SD step 20.93 vs 20.68 ms, CIFAR 11.94 vs 11.26 ms,
-// church 7.69 vs 7.71 ms - no gain inside the CUDA graphs, so the launches stay plain.
+// launch_dependents in every kernel) showed no gain inside the CUDA graphs on the previous GPU generation (not re-measured
+// on the H100), so the launches stay plain.
 template <typename... KArgs, typename... Args>
 void launch_k(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t s, Args&&... args) {
   cudaLaunchConfig_t cfg = {};
@@ -147,11 +147,12 @@ struct GemmPlan {
   int grid, mode;
 };
 
-// N-tile width.  Model (cycles per 128 x BN tile on one SM; constants fitted to tools/sweep_bn.py on B200):
+// N-tile width (<= qd::GEMM_MAX_BN).  Heuristic cost of a 128 x BN tile on one SM, in cycles (the constants are a
+// rough model, not a fit to measurements on this GPU; tools/sweep_bn.py sweeps BN per layer shape):
 //   main loop  per 128-byte k-block: max(tensor time ~ 2.1*BN, L2->SM operand delivery ~ 3.0*(128 + BN)) -- with one CTA per SM
-//              the big-K convs are bound by the operand bytes (128 + BN)*128 per k-block (profiles/r01_gemm_conv_final.txt), so wide
-//              tiles (more reuse of the A rows) win even when they leave the last wave less full;
-//   epilogue   ~ BN columns (overlaps the next tile's main loop through the double-buffered accumulators);
+//              the big-K convs are bound by the operand bytes (128 + BN)*128 per k-block, so wide tiles (more reuse of the
+//              A rows) win even when they leave the last wave less full;
+//   epilogue   ~ BN columns (overlaps the producer's loads of the next tile's operands);
 //   waves      = ceil(tiles / SMs).
 // QDIFF_BN_MODEL=wave selects the round-1 rule (waves * (BN + 24)), kept for A/B comparisons.
 int pick_bn(int N, int tiles_m, int sms, int hint, int step, long long K) {
@@ -161,7 +162,7 @@ int pick_bn(int N, int tiles_m, int sms, int hint, int step, long long K) {
   double best_cost = -1.0;
   const int n16 = (N + step - 1) / step * step;
   const double kb = (double)((K + 127) / 128);
-  for (int bn = step; bn <= 256; bn += step) {
+  for (int bn = step; bn <= qd::GEMM_MAX_BN; bn += step) {
     if (bn > n16) break;
     const long long tiles = (long long)tiles_m * ((N + bn - 1) / bn);
     const long long waves = (tiles + sms - 1) / sms;
@@ -220,17 +221,20 @@ int plan_gemm(const qd_gemm_desc* d, GemmPlan* pl) {
       return fail(QD_ERR_BAD_ARG, "gemm: geglu needs N %% 8 == 0, out_q only, plain GEMM");
   }
   a.BN = pick_bn(d->N, a.tiles_m, sms, d->bn_hint, d->geglu ? 32 : 16, (long long)d->C * d->taps * a.kdup);
+  const int bn_default = a.BN;
   // split-K candidates (see below) take the widest N tile: few tiles remain, and what is shared among the SMs is the K loop
+  // (the split-K partial kernel takes up to qd::GEMM_MAX_BN_SPLITK columns; without split-K the tile reverts to bn_default)
   static const int splitk_enabled = [] { const char* e = getenv("QDIFF_SPLITK"); return (e && !strcmp(e, "0")) ? 0 : 1; }();
   const int num_kb_all = ((d->C + qd::GEMM_BK - 1) / qd::GEMM_BK) * d->taps * a.kdup;
   const bool splitk_candidate = splitk_enabled && !d->bn_hint && !d->a_bf16 && !d->w_int4_packed && d->out && !d->out_q && !d->geglu &&
                                 !(d->N & 3) && !(d->ldo & 3) && (!d->residual || !(d->ldr & 3)) && (!d->rowvec || !(d->ld_rowvec & 3)) &&
                                 num_kb_all >= 16;
   if (splitk_candidate) {
-    const int bn_wide = d->N >= 256 ? 256 : (d->N + 15) / 16 * 16;
+    const int bn_wide = d->N >= qd::GEMM_MAX_BN_SPLITK ? qd::GEMM_MAX_BN_SPLITK : (d->N + 15) / 16 * 16;
     if (2 * a.tiles_m * ((d->N + bn_wide - 1) / bn_wide) <= sms) a.BN = bn_wide;
   }
-  if (a.BN % 16 || a.BN < 16 || a.BN > 256) return fail(QD_ERR_BAD_ARG, "gemm: bad BN %d", a.BN);
+  if (a.BN % 16 || a.BN < 16 || a.BN > qd::GEMM_MAX_BN_SPLITK || (d->bn_hint && a.BN > qd::GEMM_MAX_BN))
+    return fail(QD_ERR_BAD_ARG, "gemm: bad BN %d (16 .. %d)", a.BN, qd::GEMM_MAX_BN);
   a.tiles_n = (d->N + a.BN - 1) / a.BN;
   a.a_signed = d->a_signed; a.b_signed = 1;
 
@@ -273,25 +277,11 @@ int plan_gemm(const qd_gemm_desc* d, GemmPlan* pl) {
   }
   int rc = encode_u8_map(&pl->tmA, d->a, 4, dims, strides, box);
   if (rc) return rc;
-  // ---- B map: [w_rows][taps*C] s8, or [w_rows][taps*C/2] packed 4-bit codes (unswizzled: the unpack warps re-lay it out)
-  {
-    const int w_rows = d->w_rows > 0 ? d->w_rows : d->N;
-    if (d->w_int4_packed) {
-      if (!d->w_zero) return fail(QD_ERR_BAD_ARG, "gemm: packed INT4 weights need w_zero");
-      if (((uintptr_t)d->w) & 15) return fail(QD_ERR_BAD_ARG, "gemm: packed weights must be 16-byte aligned");
-      cuuint64_t bd[2] = {(cuuint64_t)d->taps * d->C / 2, (cuuint64_t)w_rows};
-      cuuint64_t bs[1] = {(cuuint64_t)d->taps * d->C / 2};
-      cuuint32_t bb[2] = {qd::GEMM_BK / 2, (cuuint32_t)a.BN};
-      rc = encode_u8_map(&pl->tmB, d->w, 2, bd, bs, bb, 0);
-      a.w4 = 1;
-      a.wzero = d->w_zero;
-    } else {
-      cuuint64_t bd[2] = {(cuuint64_t)d->taps * d->C * a.kdup, (cuuint64_t)w_rows};
-      cuuint64_t bs[1] = {(cuuint64_t)d->taps * d->C * a.kdup};
-      cuuint32_t bb[2] = {qd::GEMM_BK, (cuuint32_t)a.BN};
-      rc = encode_u8_map(&pl->tmB, d->w, 2, bd, bs, bb);
-    }
-    if (rc) return rc;
+  if (d->w_int4_packed) {
+    if (!d->w_zero) return fail(QD_ERR_BAD_ARG, "gemm: packed INT4 weights need w_zero");
+    if (((uintptr_t)d->w) & 15) return fail(QD_ERR_BAD_ARG, "gemm: packed weights must be 16-byte aligned");
+    a.w4 = 1;
+    a.wzero = d->w_zero;
   }
   a.out = d->out; a.ldo = d->ldo;
   a.out_q = reinterpret_cast<int8_t*>(d->out_q); a.ldq = d->ldq;
@@ -319,9 +309,9 @@ int plan_gemm(const qd_gemm_desc* d, GemmPlan* pl) {
   const int tiles = a.tiles_m * a.tiles_n;
   pl->grid = tiles < sms ? tiles : sms;
   pl->mode = gemm_mode(a);
-  // ---- split-K: short-M, long-K layers (the 4x4 / 8x8 levels: 4-48 output tiles, 90-220 k-blocks each).  A CTA's main loop
-  // runs at ~0.5 us per k-block whatever the N tile (profiles/r02_sweep_bn_small_m.txt: 50 us for BN = 32 ... 256), so the only
-  // lever is to share a tile's K loop among idle SMs.  fp32-output layers without GroupNorm slab statistics only.
+  // ---- split-K: short-M, long-K layers (the 4x4 / 8x8 levels: few output tiles, 90-220 k-blocks each).  A CTA's main loop
+  // time per k-block depends little on the N tile, so the lever is to share a tile's K loop among idle SMs.  fp32-output
+  // layers (GroupNorm slab statistics come from the finish pass).
   {
     const int num_kb = num_kb_all;
     const bool eligible = splitk_candidate && pl->mode >= 0 && 2 * tiles <= sms &&
@@ -341,6 +331,28 @@ int plan_gemm(const qd_gemm_desc* d, GemmPlan* pl) {
       }
     }
   }
+  if (a.splits <= 1 && a.BN > qd::GEMM_MAX_BN) {      // no split-K after all: the N tile of the ordinary kernels
+    a.BN = bn_default;
+    a.tiles_n = (d->N + a.BN - 1) / a.BN;
+    const int t = a.tiles_m * a.tiles_n;
+    pl->grid = t < sms ? t : sms;
+  }
+  // ---- B map: [w_rows][taps*C] s8, or [w_rows][taps*C/2] packed 4-bit codes (unswizzled: the unpack warps re-lay it out)
+  {
+    const int w_rows = d->w_rows > 0 ? d->w_rows : d->N;
+    if (d->w_int4_packed) {
+      cuuint64_t bd[2] = {(cuuint64_t)d->taps * d->C / 2, (cuuint64_t)w_rows};
+      cuuint64_t bs[1] = {(cuuint64_t)d->taps * d->C / 2};
+      cuuint32_t bb[2] = {qd::GEMM_BK / 2, (cuuint32_t)a.BN};
+      rc = encode_u8_map(&pl->tmB, d->w, 2, bd, bs, bb, 0);
+    } else {
+      cuuint64_t bd[2] = {(cuuint64_t)d->taps * d->C * a.kdup, (cuuint64_t)w_rows};
+      cuuint64_t bs[1] = {(cuuint64_t)d->taps * d->C * a.kdup};
+      cuuint32_t bb[2] = {qd::GEMM_BK, (cuuint32_t)a.BN};
+      rc = encode_u8_map(&pl->tmB, d->w, 2, bd, bs, bb);
+    }
+    if (rc) return rc;
+  }
   if (a.bf16 && pl->mode < 0)
     return fail(QD_ERR_UNSUPPORTED, "gemm: weight-only (a_bf16) layer needs a specialised epilogue (N %% 4 == 0, aligned leading dimensions)");
   memset(&pl->tmR, 0, sizeof(pl->tmR));
@@ -358,15 +370,16 @@ template <int MODE, bool W4>
 int launch_gemm_mode_w(const GemmPlan& pl, cudaStream_t s) {
   static std::atomic<unsigned long long> optin{0};
   if (int rc = ensure_smem_optin(qd::gemm_i8_kernel<MODE, W4>, 227 * 1024, optin, "gemm")) return rc;
-  constexpr int epi_warps = qd::gemm_epi_warps(MODE);
   qd::GemmArgs a = pl.args;
   const int stage_bytes = qd::gemm_stage_footprint(a.BN, W4 ? 1 : 0);
   constexpr int res_bytes = qd::gemm_res_bytes(MODE);
-  int stages = (232448 - 512 - epi_warps * qd::GEMM_EPI_TILE_BYTES - res_bytes - 1024 - 1024) / stage_bytes;
+  constexpr bool splitk = MODE >= 0 && (MODE & qd::EPI_SPLITK) != 0;
+  if (a.BN > qd::gemm_max_bn(MODE)) return fail(QD_ERR_BAD_ARG, "gemm: BN=%d exceeds %d (mode %d)", a.BN, qd::gemm_max_bn(MODE), MODE);
+  int stages = (232448 - 512 - qd::gemm_acc_tile_bytes(a.BN, splitk) - res_bytes - 1024 - 1024) / stage_bytes;
   if (stages > qd::GEMM_MAX_STAGES) stages = qd::GEMM_MAX_STAGES;
   if (stages < 2) stages = 2;
   a.stages = stages;
-  const int smem = qd::gemm_smem_layout(a.BN, stages, epi_warps, W4 ? 1 : 0, res_bytes).total;
+  const int smem = qd::gemm_smem_layout(a.BN, stages, W4 ? 1 : 0, res_bytes, splitk).total;
   if (smem > 232448) return fail(QD_ERR_UNSUPPORTED, "gemm: BN=%d needs %d bytes of shared memory for 2 stages (mode %d, w4 %d)", a.BN, smem, MODE, (int)W4);
   launch_k(qd::gemm_i8_kernel<MODE, W4>, pl.grid, qd::gemm_threads(MODE, W4), smem, s, pl.tmA, pl.tmB, pl.tmR, a);
   return check_launch("gemm_i8_kernel");
@@ -410,7 +423,7 @@ int gemm_mode(const qd::GemmArgs& a) {
 int launch_gemm(const GemmPlan& pl, cudaStream_t s) {
   using namespace qd;
   if (pl.args.splits > 1) {     // K slices -> workspace, then the epilogue pass
-    if (int rc = launch_gemm_mode<EPI_SPLITK>(pl, s)) return rc;
+    if (int rc = launch_gemm_mode_w<EPI_SPLITK, false>(pl, s)) return rc;   // split-K never takes packed INT4 weights
     launch_k(qd::splitk_finish_kernel, dim3((pl.args.N + 31) / 32, (pl.args.M + 31) / 32), 256, 0, s, pl.args);
     return check_launch("splitk_finish_kernel");
   }
@@ -472,7 +485,7 @@ int launch_quantize(const qd_quantize_desc& d, cudaStream_t s) {
 // slab / rows-per-block of the three-kernel GroupNorm: enough blocks to fill the GPU at every feature-map size
 int gn_slab_rows(int B, int HW) {
   int sms = num_sms();
-  if (sms <= 0) sms = 148;
+  if (sms <= 0) sms = 132;
   long long r = ((long long)B * HW) / (4LL * sms);
   int slab = 64;
   while (slab > 8 && slab > r) slab >>= 1;
@@ -510,12 +523,10 @@ int launch_groupnorm(const qd_groupnorm_desc& d, cudaStream_t s) {
     }();
     const long long limit = force == 1 ? 512LL * qd::GN_NU : (force == 2 ? 0 : 256LL * qd::GN_NU);
     // The one-block-per-(image, group) kernel reads cpg * 4 bytes per pixel out of every C * 4 (sector-inefficient for
-    // narrow groups) and launches B * groups blocks: it only pays in the launch-latency regime.  Measured per op on the
-    // four UNets (profiles/r02_gn_fused_vs_split.txt): the three-kernel path (statistics from the producing GEMMs'
-    // slab sums, then a coalesced apply pass) wins everywhere except maps below ~2 M elements with <= 2048 blocks
-    // (church / SD 4x4 and 8x8 levels: 10 vs 17 us); CIFAR at batch 256 (8192 blocks of 64-256 threads): 6.3 -> 1.7 ms.
-    // ... and, when the producing GEMMs left slab statistics, only below ~0.5 M elements (church 8x8 level, 1.5 M elements:
-    // 25 us fused vs 13 us for finalize-from-statistics + apply)
+    // narrow groups) and launches B * groups blocks: it only pays in the launch-latency regime.  The three-kernel path
+    // (statistics from the producing GEMMs' slab sums, then a coalesced apply pass) takes everything else: maps above ~2 M
+    // elements or with more than 2048 blocks, and above ~0.5 M elements when the producing GEMMs left slab statistics.
+    // (Thresholds from per-op timings on the previous GPU generation; not re-measured on the H100.)
     const long long elems = (long long)d.B * d.HW * d.C;
     const bool small_problem = elems <= ((d.stats_in && use_stats_env()) ? (512LL << 10) : (2LL << 20)) && (long long)d.B * d.groups <= 2048;
     if (ok && units <= limit && (force == 1 || small_problem)) {
@@ -651,15 +662,16 @@ int launch_im2col(const qd_im2col_desc& d, cudaStream_t s) {
   return check_launch("im2col_kernel");
 }
 
-template <int DQ, int DV, bool QS, bool VS, bool S16>
+template <int DQ, int DV, bool QS, bool VS, bool S16, bool F16>
 int launch_attention_inst(const qd_attention_desc& d, cudaStream_t s) {
   constexpr int MINB = (DV <= 48) ? 2 : 1;
-  auto kern = qd::qattention_kernel<DQ, DV, QS, VS, S16, MINB>;
+  auto kern = qd::qattention_kernel<DQ, DV, QS, VS, S16, MINB, F16>;
   static std::atomic<unsigned long long> optin{0};
   if (int rc = ensure_smem_optin(kern, 200 * 1024, optin, "attention")) return rc;
-  const qd::AttSmemLayout lay = qd::att_smem_layout(DQ, DV, d.Tk, d.zq != 0);
+  const bool zrk = !F16 && d.zq != 0;      // fp16 centred operands carry no zero-point cross term
+  const qd::AttSmemLayout lay = qd::att_smem_layout(DQ, DV, d.Tk, zrk);
   if (lay.total > 200 * 1024) return fail(QD_ERR_UNSUPPORTED, "attention: Tk=%d needs %d B of shared memory", d.Tk, lay.total);
-  if (d.zq != 0) {
+  if (zrk) {
     if (!d.ws) return fail(QD_ERR_BAD_ARG, "attention: workspace required when zq != 0");
     const int tk_pad = qd::att_ws_stride(d.Tk);
     launch_k(qd::att_krowsum_kernel<QS>, grid_for((long long)d.B * d.heads * tk_pad, 256), 256, 0, s, d, tk_pad, 0, 0);
@@ -671,13 +683,14 @@ int launch_attention_inst(const qd_attention_desc& d, cudaStream_t s) {
   return check_launch("qattention_kernel");
 }
 
-template <int DQ, int DV>
+// DQ: bytes of the padded QK^T reduction (8-bit codes: d rounded up to 32; F16: 2 d rounded up to 32)
+template <int DQ, int DV, bool F16 = false>
 int launch_attention_t(const qd_attention_desc& d, cudaStream_t s) {
   const bool qs = d.q_signed != 0, vs = d.v_signed != 0, s16 = d.sm_bits > 8;
-  if (qs && vs && s16) return launch_attention_inst<DQ, DV, true, true, true>(d, s);
-  if (qs && vs && !s16) return launch_attention_inst<DQ, DV, true, true, false>(d, s);
-  if (!qs && !vs && s16) return launch_attention_inst<DQ, DV, false, false, true>(d, s);
-  if (!qs && !vs && !s16) return launch_attention_inst<DQ, DV, false, false, false>(d, s);
+  if (qs && vs && s16) return launch_attention_inst<DQ, DV, true, true, true, F16>(d, s);
+  if (qs && vs && !s16) return launch_attention_inst<DQ, DV, true, true, false, F16>(d, s);
+  if (!qs && !vs && s16) return launch_attention_inst<DQ, DV, false, false, true, F16>(d, s);
+  if (!qs && !vs && !s16) return launch_attention_inst<DQ, DV, false, false, false, F16>(d, s);
   return fail(QD_ERR_UNSUPPORTED, "attention: mixed signedness q=%d v=%d", d.q_signed, d.v_signed);
 }
 
@@ -703,97 +716,85 @@ int launch_attention_smallk(const qd_attention_desc& d, cudaStream_t s) {
   return fail(QD_ERR_UNSUPPORTED, "attention: mixed signedness q=%d v=%d", d.q_signed, d.v_signed);
 }
 
-// tcgen05 path (attention_tc.cuh): d <= 112, Q/K codes in the per-head padded layout (pitch 32/64/128), dense V^T
-template <bool S16, bool MAGIC, int NSW, bool HZ, bool F16 = false>
-int launch_attention_tc_inst(const qd_attention_desc& d, const CUtensorMap& tmQ, const CUtensorMap& tmK,
-                             const CUtensorMap& tmV, int NV, int P, cudaStream_t s) {
-  auto kern = qd::qattention_tc_kernel<S16, MAGIC, NSW, HZ, F16>;
-  static std::atomic<unsigned long long> optin{0};
-  if (int rc = ensure_smem_optin(kern, NSW == 16 ? 227 * 1024 : 113 * 1024, optin, "attention_tc")) return rc;
-  const qd::AtcSmem lay = qd::atc_smem_layout(NV, P, NSW);
-  if (lay.total > (NSW == 16 ? 227 : 113) * 1024) return fail(QD_ERR_UNSUPPORTED, "attention_tc: %d B of shared memory", lay.total);
-  dim3 grid((d.Tq + qd::ATC_BM - 1) / qd::ATC_BM, d.B * d.heads);
-  launch_k(kern, grid, qd::atc_threads(NSW), lay.total, s, tmQ, tmK, tmV, d, NV, P);
-  return check_launch("qattention_tc_kernel");
-}
-template <bool S16, bool MAGIC, int NSW>
-int launch_attention_tc_hz(const qd_attention_desc& d, const CUtensorMap& tmQ, const CUtensorMap& tmK,
-                           const CUtensorMap& tmV, int NV, int P, cudaStream_t s) {
-  if (d.zq != 0) return launch_attention_tc_inst<S16, MAGIC, NSW, true>(d, tmQ, tmK, tmV, NV, P, s);
-  return launch_attention_tc_inst<S16, MAGIC, NSW, false>(d, tmQ, tmK, tmV, NV, P, s);
-}
-
-bool attention_tc_eligible(const qd_attention_desc& d) {
-  static int mode = -1;   // QDIFF_ATTENTION=mma forces the mma.sync kernel (A/B comparisons)
-  if (mode < 0) {
-    const char* e = getenv("QDIFF_ATTENTION");
-    mode = (e && !strcmp(e, "mma")) ? 0 : 1;
-  }
-  if (!mode) return false;
-  const int P = d.head_stride_q;
-  if (d.d > 112 || (d.d & 7)) return false;
-  if ((P != 32 && P != 64 && P != 128) || P < d.d * (d.qk_f16 ? 2 : 1) || d.head_stride_k != P) return false;
-  if (d.q_off != 0 || d.k_off != 0 || d.ld_q != (long long)d.heads * P || d.ld_k != (long long)d.heads * P) return false;
+// ---- wgmma attention (attention_wg.cuh): Q / K in the per-head padded layout (pitch P = 32 / 64 / 128 bytes, the K tile's
+// TMA box and swizzle span), dense V^T; d in {16, 24, 32, 40, 48, 64, 80, 96} (fp16 Q / K: d <= 64)
+bool attention_wg_eligible(const qd_attention_desc& d) {
+  static const int forced_mma = [] { const char* e = getenv("QDIFF_ATTENTION"); return (e && !strcmp(e, "mma")) ? 1 : 0; }();
+  if (forced_mma) return false;     // QDIFF_ATTENTION=mma: the mma.sync kernel (A/B comparisons)
+  const int P = d.head_stride_q, rb = d.qk_f16 ? 2 * d.d : d.d;
+  if (d.d != 16 && d.d != 24 && d.d != 32 && d.d != 40 && d.d != 48 && d.d != 64 && d.d != 80 && d.d != 96) return false;
+  if (d.qk_f16 && d.d > 64) return false;
+  // fp16 Q / K at d = 48 (LSUN-church 16x16 level) diverges from the oracle on this kernel, cause not found yet: it keeps the
+  // mma.sync kernel, which matches it
+  if (d.qk_f16 && d.d == 48) return false;
+  if ((P != 32 && P != 64 && P != 128) || P < rb || d.head_stride_k != P) return false;
+  if (d.q_off != 0 || d.k_off != 0 || (d.ld_k & 15) || (((uintptr_t)d.k) & 15) || (((uintptr_t)d.vt) & 15)) return false;
   if (d.v_off != 0 || d.head_stride_v != d.d || d.v_batch_stride != (long long)d.heads * d.d * d.ld_vt) return false;
-  if (d.out && ((d.ld_out & 3) || (((uintptr_t)d.out) & 15))) return false;
-  if (d.out_q && (d.ld_out_q & 3)) return false;
+  if (d.zq != 0 && !d.qk_f16 && !d.ws) return false;
   return true;
 }
 
-int launch_attention_tc(const qd_attention_desc& d, cudaStream_t s) {
-  const int NV = (d.d + 1 + 15) / 16 * 16;
+template <int DQ, int DV, bool QS, bool VS, bool S16, bool F16>
+int launch_attention_wg_inst(const qd_attention_desc& d, cudaStream_t s) {
+  auto kern = qd::qattention_wg_kernel<DQ, DV, QS, VS, S16, F16>;
   const int P = d.head_stride_q;
-  CUtensorMap tmQ, tmK, tmV;
+  const qd::AtwSmem lay = qd::atw_smem(P, qd::atw_nv(DV));
+  static std::atomic<unsigned long long> optin{0};
+  if (int rc = ensure_smem_optin(kern, 227 * 1024, optin, "attention_wg")) return rc;
+  CUtensorMap tmK, tmV;
   {
-    cuuint64_t dims[2] = {(cuuint64_t)d.ld_q, (cuuint64_t)d.B * d.Tq};
-    cuuint64_t strides[1] = {(cuuint64_t)d.ld_q};
-    cuuint32_t box[2] = {(cuuint32_t)P, 128};
-    int rc = encode_u8_map(&tmQ, d.q, 2, dims, strides, box, P);
-    if (rc) return rc;
-    dims[1] = (cuuint64_t)d.B * d.Tk;
-    rc = encode_u8_map(&tmK, d.k, 2, dims, strides, box, P);
-    if (rc) return rc;
+    cuuint64_t dims[2] = {(cuuint64_t)d.ld_k, (cuuint64_t)d.B * d.Tk};
+    cuuint64_t strides[1] = {(cuuint64_t)d.ld_k};
+    cuuint32_t box[2] = {(cuuint32_t)P, (cuuint32_t)qd::ATT_BN};
+    if (int rc = encode_u8_map(&tmK, d.k, 2, dims, strides, box, P)) return rc;
   }
-  cuuint64_t dims[2] = {(cuuint64_t)d.ld_vt, (cuuint64_t)d.B * d.heads * d.d};
-  cuuint64_t strides[1] = {(cuuint64_t)d.ld_vt};
-  cuuint32_t box[2] = {128, (cuuint32_t)d.d};
-  int rc = encode_u8_map(&tmV, d.vt, 2, dims, strides, box);
-  if (rc) return rc;
-  static const int two_cta = [] { const char* e = getenv("QDIFF_ATTN_2CTA"); return (e && !strcmp(e, "0")) ? 0 : 1; }();
-  if (d.qk_f16) {      // fp16 (code - zero_point) operands: no zero-point correction pass
-    const bool small16 = two_cta && P <= 64 && NV <= 64 && (long long)d.Tq * d.Tk <= (1LL << 21) &&
-                         qd::atc_smem_layout(NV, P, 8).total <= 113 * 1024;
-    if (small16) {
-      if (d.sm_bits > 8) return launch_attention_tc_inst<true, true, 8, false, true>(d, tmQ, tmK, tmV, NV, P, s);
-      return launch_attention_tc_inst<false, true, 8, false, true>(d, tmQ, tmK, tmV, NV, P, s);
-    }
-    if (d.sm_bits > 8) return launch_attention_tc_inst<true, true, 16, false, true>(d, tmQ, tmK, tmV, NV, P, s);
-    return launch_attention_tc_inst<false, true, 16, false, true>(d, tmQ, tmK, tmV, NV, P, s);
+  {
+    cuuint64_t dims[2] = {(cuuint64_t)d.ld_vt, (cuuint64_t)d.B * d.heads * d.d};
+    cuuint64_t strides[1] = {(cuuint64_t)d.ld_vt};
+    cuuint32_t box[2] = {(cuuint32_t)qd::ATT_BN, (cuuint32_t)d.d};
+    if (int rc = encode_u8_map(&tmV, d.vt, 2, dims, strides, box, 64)) return rc;
   }
-  if (d.zq != 0) {
-    if (!d.ws) return fail(QD_ERR_BAD_ARG, "attention: workspace required when zq != 0");
+  if (!F16 && d.zq != 0) {
     const int tk_pad = qd::att_ws_stride(d.Tk);
-    const int bias = d.d <= 64 ? 0x4B400000 : 0;   // MAGIC variant of the kernel (see attention_tc.cuh)
-    if (d.q_signed) launch_k(qd::att_krowsum_kernel<true>, grid_for((long long)d.B * d.heads * tk_pad, 256), 256, 0, s, d, tk_pad, 1, bias);
-    else launch_k(qd::att_krowsum_kernel<false>, grid_for((long long)d.B * d.heads * tk_pad, 256), 256, 0, s, d, tk_pad, 1, bias);
-    rc = check_launch("att_krowsum_kernel");
-    if (rc) return rc;
+    launch_k(qd::att_krowsum_kernel<QS>, grid_for((long long)d.B * d.heads * tk_pad, 256), 256, 0, s, d, tk_pad, 0, 0);
+    if (int rc = check_launch("att_krowsum_kernel")) return rc;
   }
-  const bool s16 = d.sm_bits > 8, magic = d.d <= 64;
-  // two co-resident CTAs per SM (8 softmax warps each) when the 256-column TMEM layout and 113 KB of shared memory suffice;
-  // QDIFF_ATTN_2CTA=0 forces the one-CTA (16 softmax warps) configuration (A/B comparisons)
-  // measured (tools/prof_attn.py, B=16 x 8 heads, d=40): Tq=Tk=1024: 143 us vs 150 us with one CTA per SM; Tq=Tk=4096: 1845
-  // vs 1750 us (the long problem is throughput-bound on MUFU + issue, the single S slot costs more than co-residency gains)
-  const bool small = two_cta && P <= 64 && NV <= 64 && magic && (long long)d.Tq * d.Tk <= (1LL << 21) &&
-                     qd::atc_smem_layout(NV, P, 8).total <= 113 * 1024;
-  if (small) {
-    if (s16) return launch_attention_tc_hz<true, true, 8>(d, tmQ, tmK, tmV, NV, P, s);
-    return launch_attention_tc_hz<false, true, 8>(d, tmQ, tmK, tmV, NV, P, s);
+  dim3 grid((d.Tq + qd::ATT_BM - 1) / qd::ATT_BM, d.B * d.heads);
+  launch_k(kern, grid, qd::ATW_THREADS, lay.total, s, tmK, tmV, d, P);
+  return check_launch("qattention_wg_kernel");
+}
+
+template <int DQ, int DV, bool F16>
+int launch_attention_wg_t(const qd_attention_desc& d, cudaStream_t s) {
+  const bool qs = d.q_signed != 0, vs = d.v_signed != 0, s16 = d.sm_bits > 8;
+  if (qs && vs && s16) return launch_attention_wg_inst<DQ, DV, true, true, true, F16>(d, s);
+  if (qs && vs && !s16) return launch_attention_wg_inst<DQ, DV, true, true, false, F16>(d, s);
+  if (!qs && !vs && s16) return launch_attention_wg_inst<DQ, DV, false, false, true, F16>(d, s);
+  if (!qs && !vs && !s16) return launch_attention_wg_inst<DQ, DV, false, false, false, F16>(d, s);
+  return fail(QD_ERR_UNSUPPORTED, "attention: mixed signedness q=%d v=%d", d.q_signed, d.v_signed);
+}
+
+int launch_attention_wg(const qd_attention_desc& d, cudaStream_t s) {
+  if (d.qk_f16) {
+    switch (d.d) {
+      case 16: return launch_attention_wg_t<32, 16, true>(d, s);
+      case 24: return launch_attention_wg_t<64, 24, true>(d, s);
+      case 32: return launch_attention_wg_t<64, 32, true>(d, s);
+      case 40: return launch_attention_wg_t<96, 40, true>(d, s);
+      case 48: return launch_attention_wg_t<96, 48, true>(d, s);
+      default: return launch_attention_wg_t<128, 64, true>(d, s);
+    }
   }
-  if (s16 && magic) return launch_attention_tc_hz<true, true, 16>(d, tmQ, tmK, tmV, NV, P, s);
-  if (s16 && !magic) return launch_attention_tc_hz<true, false, 16>(d, tmQ, tmK, tmV, NV, P, s);
-  if (!s16 && magic) return launch_attention_tc_hz<false, true, 16>(d, tmQ, tmK, tmV, NV, P, s);
-  return launch_attention_tc_hz<false, false, 16>(d, tmQ, tmK, tmV, NV, P, s);
+  switch (d.d) {
+    case 16: return launch_attention_wg_t<32, 16, false>(d, s);
+    case 24: return launch_attention_wg_t<32, 24, false>(d, s);
+    case 32: return launch_attention_wg_t<32, 32, false>(d, s);
+    case 40: return launch_attention_wg_t<64, 40, false>(d, s);
+    case 48: return launch_attention_wg_t<64, 48, false>(d, s);
+    case 64: return launch_attention_wg_t<64, 64, false>(d, s);
+    case 80: return launch_attention_wg_t<96, 80, false>(d, s);
+    default: return launch_attention_wg_t<96, 96, false>(d, s);
+  }
 }
 
 int launch_attention(const qd_attention_desc& d, cudaStream_t s) {
@@ -806,16 +807,23 @@ int launch_attention(const qd_attention_desc& d, cudaStream_t s) {
   if ((d.q_off | d.head_stride_q | (int)d.ld_q) & 3) return fail(QD_ERR_UNSUPPORTED, "attention: q needs 4-byte alignment");
   if ((d.k_off | d.head_stride_k | (int)d.ld_k | d.d) & 7) return fail(QD_ERR_UNSUPPORTED, "attention: k rows need 8-byte alignment");
   if (d.out && (d.ld_out % 2)) return fail(QD_ERR_UNSUPPORTED, "attention: ld_out");
-  if (d.qk_f16) {
-    if (d.d > 64 || !attention_tc_eligible(d))
-      return fail(QD_ERR_UNSUPPORTED, "attention: qk_f16 needs the tcgen05 layout (d <= 64, per-head pitch 32/64/128 bytes >= 2 * d)");
-    return launch_attention_tc(d, s);
+  if (d.qk_f16) {      // fp16 centred-code Q / K (QK^T on f16 x f16 -> f32 MMAs, exact), d <= 64, any Tk
+    if (attention_wg_eligible(d)) return launch_attention_wg(d, s);
+    switch (d.d) {
+      case 16: return launch_attention_t<32, 16, true>(d, s);
+      case 24: return launch_attention_t<64, 24, true>(d, s);
+      case 32: return launch_attention_t<64, 32, true>(d, s);
+      case 40: return launch_attention_t<96, 40, true>(d, s);
+      case 48: return launch_attention_t<96, 48, true>(d, s);
+      case 64: return launch_attention_t<128, 64, true>(d, s);
+      default: return fail(QD_ERR_UNSUPPORTED, "attention: qk_f16 needs d in {16, 24, 32, 40, 48, 64} (got %d)", d.d);
+    }
   }
   if (d.Tk <= 96 && (d.d == 40 || d.d == 80)) {
     static const bool off = [] { const char* e = getenv("QDIFF_ATTENTION"); return e && !strcmp(e, "nosmallk"); }();
     if (!off) return d.d == 40 ? launch_attention_smallk<64, 40>(d, s) : launch_attention_smallk<96, 80>(d, s);
   }
-  if (attention_tc_eligible(d)) return launch_attention_tc(d, s);
+  if (attention_wg_eligible(d)) return launch_attention_wg(d, s);
   switch (d.d) {
     case 16: return launch_attention_t<32, 16>(d, s);
     case 24: return launch_attention_t<32, 24>(d, s);

@@ -1,4 +1,4 @@
-// INT8 tcgen05 GEMM / implicit-GEMM conv3x3 for sm_100a.
+// INT8 wgmma GEMM / implicit-GEMM conv3x3 for sm_90a.
 //
 // Realises the reference's QuantModule.forward (qdiff/quant_layer.py:248-279) as true integer
 // compute:   y[m,n] = scale[n] * (sum_k xq[m,k]*ws[n,k] - corr[cls(m)][n]) + bias[n] (+ fused adds)
@@ -7,19 +7,18 @@
 // because the reference pads with real zeros AFTER de-quantisation, SURVEY Appendix A.3).
 //
 // Structure (one CTA per SM, persistent, warp-specialised):
-//   warp 0   : TMA producer  (A tile 128 x 128 B, B tile BN x 128 B, 128B swizzle, mbarrier ring)
-//   warp 1   : MMA issuer    (tcgen05.mma.kind::i8, M=128, N=BN, K=32 per instruction, int32 acc in TMEM)
-//   warp 2   : TMEM allocator (512 columns: two accumulator stages of up to 256 columns)
+//   warp 0   : TMA producer  (A tile 128 x 128 B, B tile BN x 128 B, 128B swizzle, mbarrier ring); warp 1 idle
 //   warps 2-3 and the LAST two warps: INT4 unpack (W4 variant only: packed 4-bit weight codes staged by TMA -> swizzled
 //              s8 operand tile; four warps = one per scheduler)
-//   warps 4+ : epilogue, 8 or 16 warps by MODE (tcgen05.ld -> smem transpose -> zero-point correction / scale /
-//                             bias / adds / GEGLU -> coalesced fp32 or requantised stores)
+//   warps 4-11: two consumer warpgroups.  Warpgroup g issues wgmma m64nNk32 (int32 accumulators in registers) for rows
+//              [64g, 64g + 64) of the tile, the N tile as 64-column sub-blocks; after the K loop both warpgroups write
+//              their accumulators to a shared-memory tile, and the same eight warps run the epilogue from it
+//              (zero-point correction / scale / bias / adds / GEGLU -> coalesced fp32 or requantised stores).
+//   While the consumers run the epilogue, the producer already streams the next tile's operands into the ring.
 //
 // The kernel is templated on the epilogue MODE so the hot variants carry no runtime flag tests
-// (the first version with runtime flags was instruction-issue / I-cache bound in the epilogue:
-// profiles/r01_gemm_epilogue_v1.txt, r01_gemm_smallk.txt).  MODE = -1 keeps every runtime option (ragged N, both
-// outputs).  What bounds it: the K >= 2880 convs are limited by L2->SM operand delivery (profiles/
-// r01_gemm_conv_final.txt: 42 % tensor activity at the L2 slice cap), the small-K linears by their epilogue.
+// (a version with runtime flags was instruction-issue / I-cache bound in the epilogue).  MODE = -1 keeps every runtime
+// option (ragged N, both outputs).
 #pragma once
 #include "ptx.cuh"
 #include "quant_math.cuh"
@@ -30,24 +29,17 @@ namespace qd {
 
 constexpr int GEMM_BM = 128;
 constexpr int GEMM_BK = 128;  // bytes == int8 elements per k-block (one 128B swizzle row)
-// warps 0-3: TMA / MMA / TMEM alloc / idle; then EPI_WARPS epilogue warps (8 or 16): EPI_WARPS/4 warps per TMEM lane
-// quarter, taking 32-column chunks round-robin.  The instruction-bound epilogues whose register footprint
-// allows it (GEGLU, transposed V^T: <= 102 registers at 640 threads) run with 16 warps = 4 per scheduler.
-__host__ __device__ constexpr int gemm_epi_warps(int MODE) {
-  // 16 warps: EPI_GEGLU | EPI_TRANS, plain requantising epilogues (EPI_OUT_Q without residual / rowvec), and - round 2 -
-  // the fp32-output epilogues of the plain GEMMs (to_out / ff.net.2 / proj_out / proj_in: EPI_OUT_F32 without EPI_CONV or
-  // EPI_ROWVEC).  Those are bound by memory latency, not instructions: with 8 warps x 4 rows x 16 B of residual per
-  // thread an SM had 16 KB of loads in flight and the kernels sat at 3.5 TB/s with 17 % issue activity
-  // (profiles/r02_gemm_smallk_before.txt); twice the warps = twice the bytes in flight.
-  if (MODE < 0) return 8;
-  if ((MODE & (32 | 64)) != 0) return 16;
-  if ((MODE & 16) != 0 && (MODE & (2 | 4)) == 0) return 16;
-  if ((MODE & 8) != 0 && (MODE & (2 | 4 | 128)) == 0) return 16;
-  return 8;
-}
-// Residual operand through TMA (round 2): the plain-GEMM epilogues that add a residual (to_out / ff.net.2 / proj_out:
-// EPI_RESIDUAL without EPI_CONV) were bound by the latency of their residual loads: per 32x32 chunk a warp issued 4 rows
-// of LDG.128, waited a DRAM round trip, stored, issued the next 4 rows, waited again (3.3-3.5 TB/s, 17 % issue activity).
+// BN <= 128: the two consumer warpgroups hold 128 x BN int32 accumulators in registers (BN / 2 per thread) next to the
+// epilogue's working set, and the accumulator tile in shared memory is 128 x BN x 4 bytes.  The split-K partial kernel
+// (EPI_SPLITK) stores its raw accumulators straight from the registers, needs no accumulator tile and takes BN <= 256.
+constexpr int GEMM_MAX_BN = 128;
+constexpr int GEMM_MAX_BN_SPLITK = 256;
+// warps 0-3: TMA producer / idle (unpack warps 2-3 in the W4 variant); then the two consumer warpgroups (8 warps), which
+// are also the epilogue warps: warp (4 + 4h + q) finalises rows [32q, 32q + 32) of the tile, 32-column chunks h, h + 2, ...
+__host__ __device__ constexpr int gemm_epi_warps(int MODE) { return (void)MODE, 8; }
+// Residual operand through TMA: the plain-GEMM epilogues that add a residual (to_out / ff.net.2 / proj_out: EPI_RESIDUAL
+// without EPI_CONV) are bound by the latency of their residual loads when each warp issues 4 rows of LDG.128, waits a DRAM
+// round trip, stores, and issues the next 4 rows.
 // Now every epilogue warp owns a ring of GEMM_RES_NBUF 4 KB buffers and keeps the residual sub-tiles of its NEXT work items
 // (tile, chunk) in flight as cp.async.bulk.tensor loads while it finalises the current one.
 constexpr int GEMM_RES_NBUF = 3;
@@ -55,11 +47,16 @@ __host__ __device__ constexpr bool gemm_res_tma(int MODE) { return MODE >= 0 && 
 __host__ __device__ constexpr int gemm_res_bytes(int MODE) {
   return gemm_res_tma(MODE) ? gemm_epi_warps(MODE) * GEMM_RES_NBUF * 4096 : 0;
 }
-// W4 (packed INT4 weights): two more warps behind the epilogue warps join warps 2-3 as unpack warps
+// W4 (packed INT4 weights): two more warps behind the consumer warps join warps 2-3 as unpack warps
 __host__ __device__ constexpr int gemm_threads(int MODE, bool W4 = false) { return (4 + gemm_epi_warps(MODE) + (W4 ? 2 : 0)) * 32; }
 constexpr int GEMM_A_STAGE_BYTES = GEMM_BM * GEMM_BK;
 constexpr int GEMM_MAX_STAGES = 8;
-constexpr int GEMM_EPI_TILE_BYTES = 32 * 128;  // per-epilogue-warp staging tile (32 rows x 32 int32)
+constexpr int GEMM_EPI_TILE_BYTES = 32 * 128;  // one 32 x 32 int32 chunk of the accumulator tile
+// accumulator tile: 4 row quarters x ceil(BN / 32) column chunks of 32 rows x 128 B, 16-byte units XOR-swizzled by row & 7
+// (conflict-free for the epilogue's row-wise and column-quad-wise reads)
+__host__ __device__ inline int gemm_acc_tile_bytes(int BN, bool splitk = false) {
+  return splitk ? 0 : 4 * ((BN + 31) / 32) * GEMM_EPI_TILE_BYTES;
+}
 
 // epilogue MODE bits (MODE < 0: generic)
 constexpr int EPI_CORR = 1;       // subtract zero-point correction
@@ -73,13 +70,14 @@ constexpr int EPI_CONV = 128;     // 3x3 conv (taps == 9); with EPI_CORR the cor
 constexpr int EPI_RESTMA = 256;   // with EPI_RESIDUAL: residual sub-tiles arrive through the per-warp TMA ring (short-K GEMMs)
 constexpr int EPI_BF16 = 512;     // weight-only layers: bfloat16 x3 activation planes x bfloat16 weight codes, fp32 accumulators
 constexpr int EPI_SPLITK = 1024;  // split-K partial: raw int32 accumulators of one K slice -> ws[split][M][N] (splitk_finish_kernel applies the epilogue)
+__host__ __device__ constexpr int gemm_max_bn(int MODE) { return (MODE >= 0 && (MODE & EPI_SPLITK) != 0) ? GEMM_MAX_BN_SPLITK : GEMM_MAX_BN; }
 
 struct GemmArgs {
   int M, N;            // logical output rows / columns (columns >= N are masked)
   int C;               // reduction length per tap (multiple of 32)
   int taps;            // 1 = plain GEMM, 9 = 3x3 conv (stride 1, pad 1)
   int kdup;            // 1, or 2: two weight segments over the same activation (8-bit weights as wa + wb, qd_gemm_desc.k_dup)
-  int BN;              // N tile (multiple of 16, <= 256)
+  int BN;              // N tile (multiple of 16, <= GEMM_MAX_BN)
   int tiles_m, tiles_n;
   int stages;
   // conv geometry (taps == 9): activations are NHWC, tile = bn images x bh rows x W columns = 128 pixels (W > 128: a
@@ -129,7 +127,7 @@ struct GemmSmemLayout {
   int stage_bytes;
   int pack_off;   // packed-INT4 B tiles, stages x BN x 64 bytes (w4 only)
   int bar_offset;
-  int stage_off;  // epilogue staging tiles (one per epilogue warp)
+  int stage_off;  // accumulator tile (gemm_acc_tile_bytes)
   int res_off;    // residual ring (GEMM_RES_NBUF x 4 KB per epilogue warp; residual-by-TMA modes only)
   int total;
 };
@@ -138,7 +136,7 @@ __host__ __device__ inline int gemm_stage_footprint(int BN, int w4) {
   return GEMM_A_STAGE_BYTES + BN * GEMM_BK + (w4 ? BN * (GEMM_BK / 2) : 0);
 }
 
-__host__ __device__ inline GemmSmemLayout gemm_smem_layout(int BN, int stages, int epi_warps, int w4 = 0, int res_bytes = 0) {
+__host__ __device__ inline GemmSmemLayout gemm_smem_layout(int BN, int stages, int w4 = 0, int res_bytes = 0, bool splitk = false) {
   GemmSmemLayout l;
   l.stage_bytes = GEMM_A_STAGE_BYTES + BN * GEMM_BK;
   l.pack_off = l.stage_bytes * stages;
@@ -146,7 +144,7 @@ __host__ __device__ inline GemmSmemLayout gemm_smem_layout(int BN, int stages, i
   l.stage_off = l.bar_offset + 512;
   // the ring buffers are TMA targets with the 128-byte swizzle: the pattern is a function of the shared-memory ADDRESS
   // (bits 4-6 ^= bits 7-9), so they must start on a 1024-byte boundary for "chunk ^ (row & 7)" to address them
-  l.res_off = (l.stage_off + epi_warps * GEMM_EPI_TILE_BYTES + 1023) / 1024 * 1024;
+  l.res_off = (l.stage_off + gemm_acc_tile_bytes(BN, splitk) + 1023) / 1024 * 1024;
   l.total = l.res_off + res_bytes + 1024;  // + alignment slack
   return l;
 }
@@ -169,7 +167,17 @@ __device__ __forceinline__ void gemm_row_meta(const GemmArgs& p, int m, int& cls
 // The consumer's activation quantizer (qdiff/quant_layer.py:82-88) is applied with quant_math.cuh's QuantK,
 // built ONCE per thread before the tile loop: building it (MUFU.RCP + Newton + slow-path test) inside the
 // per-row code, where the compiler will not hoist it out of the `m < M` conditional, tripled the instruction
-// count of the requantising epilogues (profiles/r01_gemm_smallk.txt).
+// count of the requantising epilogues.
+
+// Row `row` (columns 0 .. NC-1) of a 32 x 32 chunk of the accumulator tile.
+template <int NC>
+__device__ __forceinline__ void gemm_acc_row(const uint8_t* chunk, int row, uint32_t (&v)[NC]) {
+#pragma unroll
+  for (int j = 0; j < NC / 4; ++j) {
+    const uint4 u = *reinterpret_cast<const uint4*>(chunk + row * 128 + ((j ^ (row & 7)) << 4));
+    v[4 * j] = u.x; v[4 * j + 1] = u.y; v[4 * j + 2] = u.z; v[4 * j + 3] = u.w;
+  }
+}
 
 // Thread-per-row epilogue (used for the transposed V^T code output: consecutive lanes = consecutive
 // tokens, so each per-column byte store of the warp fills one 32 B sector).
@@ -349,6 +357,79 @@ __device__ __forceinline__ void gemm_finalise4(const GemmArgs& p, const QuantK& 
   }
 }
 
+// One k-block (128 bytes = four 32-byte K steps of every row) of a consumer warpgroup: acc[s] (+)= A[64 rows] *
+// B[rows 64s .. 64s + 63]^T for the NF full 64-column sub-blocks, and a last sub-block TAIL (0, 16, 32 or 48) columns
+// wide.  All compile-time: the wgmma sequence is straight-line code (a wgmma under a run-time branch is serialised by
+// ptxas).  A partial last k-block of a tap needs no special case: its A columns beyond C are zero-filled by TMA, so the
+// extra K steps add exact zeros.
+template <bool BF16, bool SIGNED, int NF, int TAIL, int NS, typename T>
+__device__ __forceinline__ void gemm_wgmma_kblock(T (&acc)[NS][32], uint64_t da, uint64_t db, uint32_t scale_first) {
+#pragma unroll
+  for (int j = 0; j < 4; ++j) {
+    const uint32_t sd = j ? 1u : scale_first;
+    const uint64_t a = da + (uint64_t)(2 * j);       // +32 bytes inside the 128B swizzle row
+#pragma unroll
+    for (int s = 0; s <= NF; ++s) {
+      const uint64_t b = db + (uint64_t)((s * 64 * GEMM_BK) >> 4) + (uint64_t)(2 * j);
+      if (s < NF) {
+        if constexpr (BF16) wgmma_bf16_n64(acc[s < NS ? s : 0], a, b, sd);
+        else if constexpr (SIGNED) wgmma_s8s8_n64(acc[s < NS ? s : 0], a, b, sd);
+        else wgmma_u8s8_n64(acc[s < NS ? s : 0], a, b, sd);
+      } else if constexpr (TAIL != 0) {
+        constexpr int t = NF < NS ? NF : 0;
+        if constexpr (BF16) {
+          if constexpr (TAIL == 48) wgmma_bf16_n48(acc[t], a, b, sd);
+          else if constexpr (TAIL == 32) wgmma_bf16_n32(acc[t], a, b, sd);
+          else wgmma_bf16_n16(acc[t], a, b, sd);
+        } else if constexpr (SIGNED) {
+          if constexpr (TAIL == 48) wgmma_s8s8_n48(acc[t], a, b, sd);
+          else if constexpr (TAIL == 32) wgmma_s8s8_n32(acc[t], a, b, sd);
+          else wgmma_s8s8_n16(acc[t], a, b, sd);
+        } else {
+          if constexpr (TAIL == 48) wgmma_u8s8_n48(acc[t], a, b, sd);
+          else if constexpr (TAIL == 32) wgmma_u8s8_n32(acc[t], a, b, sd);
+          else wgmma_u8s8_n16(acc[t], a, b, sd);
+        }
+      }
+    }
+  }
+}
+
+template <int NF_, int TAIL_, bool SIGNED_>
+struct GemmNCfg {
+  static constexpr int NF = NF_, TAIL = TAIL_;
+  static constexpr bool SIGNED = SIGNED_;
+};
+// Calls f(GemmNCfg<BN / 64, BN % 64, signed>{}) for the run-time N tile BN (a multiple of 16, <= 64 * NS).
+template <int NS, bool S, typename F>
+__device__ __forceinline__ void gemm_dispatch_bn(int BN, F&& f) {
+  switch (BN >> 4) {
+    case 1: f(GemmNCfg<0, 16, S>{}); break;
+    case 2: f(GemmNCfg<0, 32, S>{}); break;
+    case 3: f(GemmNCfg<0, 48, S>{}); break;
+    case 4: f(GemmNCfg<1, 0, S>{}); break;
+    case 5: f(GemmNCfg<1, 16, S>{}); break;
+    case 6: f(GemmNCfg<1, 32, S>{}); break;
+    case 7: f(GemmNCfg<1, 48, S>{}); break;
+    default:
+      if constexpr (NS == 2) {
+        f(GemmNCfg<2, 0, S>{});
+      } else {
+        switch (BN >> 4) {
+          case 8: f(GemmNCfg<2, 0, S>{}); break;
+          case 9: f(GemmNCfg<2, 16, S>{}); break;
+          case 10: f(GemmNCfg<2, 32, S>{}); break;
+          case 11: f(GemmNCfg<2, 48, S>{}); break;
+          case 12: f(GemmNCfg<3, 0, S>{}); break;
+          case 13: f(GemmNCfg<3, 16, S>{}); break;
+          case 14: f(GemmNCfg<3, 32, S>{}); break;
+          case 15: f(GemmNCfg<3, 48, S>{}); break;
+          default: f(GemmNCfg<4, 0, S>{}); break;
+        }
+      }
+  }
+}
+
 // W4: packed-INT4 weight variant (compile-time, so the s8 kernels carry none of the unpack role's code: with a
 // run-time flag the register allocation of the epilogue changed and the default path lost 8 %).
 template <int MODE, bool W4 = false>
@@ -363,15 +444,14 @@ gemm_i8_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   constexpr int EPI_WARPS = gemm_epi_warps(MODE);
   constexpr int CSTEP = 32 * (EPI_WARPS / 4);   // column stride between the chunks of one epilogue warp
   constexpr bool RES_TMA = gemm_res_tma(MODE);
-  const GemmSmemLayout lay = gemm_smem_layout(p.BN, p.stages, EPI_WARPS, W4 ? 1 : 0, gemm_res_bytes(MODE));
+  constexpr bool SPLITK = MODE >= 0 && (MODE & EPI_SPLITK) != 0;
+  constexpr int NS = gemm_max_bn(MODE) / 64;     // 64-column accumulator sub-blocks
+  const GemmSmemLayout lay = gemm_smem_layout(p.BN, p.stages, W4 ? 1 : 0, gemm_res_bytes(MODE), SPLITK);
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + lay.bar_offset);
   uint64_t* full_bar = bars;                          // [stages]
-  uint64_t* empty_bar = bars + GEMM_MAX_STAGES;       // [stages]
-  uint64_t* tmem_full = bars + 2 * GEMM_MAX_STAGES;   // [2]
-  uint64_t* tmem_empty = tmem_full + 2;               // [2]
-  uint64_t* ready_bar = tmem_empty + 2;               // [stages] (w4: B tile unpacked, stage ready for the MMA)
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(ready_bar + GEMM_MAX_STAGES);
-  uint64_t* res_bar = ready_bar + GEMM_MAX_STAGES + 1;   // [EPI_WARPS][GEMM_RES_NBUF] (residual ring, RES_TMA only)
+  uint64_t* empty_bar = bars + GEMM_MAX_STAGES;       // [stages] (one arrival per consumer warpgroup)
+  uint64_t* ready_bar = bars + 2 * GEMM_MAX_STAGES;   // [stages] (w4: B tile unpacked, stage ready for the MMA)
+  uint64_t* res_bar = bars + 3 * GEMM_MAX_STAGES;     // [EPI_WARPS][GEMM_RES_NBUF] (residual ring, RES_TMA only)
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -389,26 +469,15 @@ gemm_i8_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   if (warp == 1 && lane == 0) {
     for (int s = 0; s < p.stages; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 1);
+      mbar_init(&empty_bar[s], EPI_WARPS / 4);
       if constexpr (W4) mbar_init(&ready_bar[s], 4);    // one arrival per unpack warp
-    }
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(&tmem_full[s], 1);
-      mbar_init(&tmem_empty[s], EPI_WARPS);
     }
     if constexpr (RES_TMA)
       for (int s = 0; s < EPI_WARPS * GEMM_RES_NBUF; ++s) mbar_init(&res_bar[s], 1);
     fence_mbar_init();
     fence_proxy_async();
   }
-  if (warp == 2) {
-    tmem_alloc(tmem_ptr, 512);
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
 
   if (warp == 0) {
     // ===================== TMA producer =====================
@@ -455,43 +524,7 @@ gemm_i8_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         }
       }
     }
-  } else if (warp == 1) {
-    // ===================== MMA issuer =====================
-    if (lane == 0) {
-      constexpr bool BF16 = MODE >= 0 && (MODE & EPI_BF16) != 0;
-      const uint32_t idesc = BF16 ? make_idesc_bf16(GEMM_BM, p.BN) : make_idesc_i8(GEMM_BM, p.BN, p.a_signed, p.b_signed);
-      int stage = 0;
-      uint32_t phase = 0;
-      int acc = 0;
-      uint32_t acc_phase = 0;
-      for (int item = blockIdx.x; item < num_tiles; item += gridDim.x) {
-        const int kb0 = (item % splits) * kb_slice;
-        const int kb1 = min(num_kb_all, kb0 + kb_slice);
-        mbar_wait(&tmem_empty[acc], acc_phase ^ 1);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + (uint32_t)(acc * 256);
-        for (int kb = kb0; kb < kb1; ++kb) {
-          const int kc = kb % kb_per_tap;
-          const int rem = p.C - kc * GEMM_BK;
-          const int nmma = rem >= GEMM_BK ? 4 : (rem >> 5);
-          mbar_wait(W4 ? &ready_bar[stage] : &full_bar[stage], phase);
-          tc_fence_after();
-          const uint32_t sa = smem_u32(smem + (size_t)stage * lay.stage_bytes);
-          const uint64_t da = make_smem_desc_sw128(sa);
-          const uint64_t db = make_smem_desc_sw128(sa + GEMM_A_STAGE_BYTES);
-          for (int j = 0; j < nmma; ++j) {
-            // advance 32 bytes (one K=32 slice) inside the 128B swizzle row: +2 in 16-byte units
-            if constexpr (BF16) umma_bf16(d_tmem, da + (uint64_t)(2 * j), db + (uint64_t)(2 * j), idesc, ((kb - kb0) | j) ? 1u : 0u);
-            else umma_i8(d_tmem, da + (uint64_t)(2 * j), db + (uint64_t)(2 * j), idesc, ((kb - kb0) | j) ? 1u : 0u);
-          }
-          umma_commit(&empty_bar[stage]);
-          if (++stage == p.stages) { stage = 0; phase ^= 1; }
-        }
-        umma_commit(&tmem_full[acc]);
-        if (++acc == 2) { acc = 0; acc_phase ^= 1; }
-      }
-    }
-  } else if (warp < 4 || warp >= 4 + EPI_WARPS) {
+  } else if (warp == 2 || warp == 3 || warp >= 4 + EPI_WARPS) {
     // ===================== INT4 unpack (warps 2, 3 and the two warps behind the epilogue warps; W4 only) ==========
     // 128 threads = 32 rows x 4 sixteen-byte pieces per pass.  A piece holds 32 codes (k = 32j .. 32j+31 of the
     // k-block) and becomes two 16-byte chunks of the row in the 128B-swizzled s8 tile the MMA descriptor expects
@@ -545,16 +578,24 @@ gemm_i8_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         }
       }
     }
-  } else {
-    // ===================== epilogue =====================
-    // TMEM gives each thread one accumulator ROW; storing that way makes every warp store touch 32
-    // different rows (16 B each).  Row-major outputs therefore go through a per-warp 32x32 int32
-    // staging tile in shared memory (128 B rows, 16 B chunks XOR-swizzled by row&7: conflict-free both
-    // ways) and are finalised in the transposed mapping: 8 lanes x 16 B = one full 128 B line per row,
-    // 4 rows per instruction, per-column parameters loaded once per thread per chunk.
-    const int q = warp & 3;  // TMEM lane quarter this warp may access
-    const int half = (warp - 4) >> 2;   // which of the two warps sharing this lane quarter
-    uint8_t* stg = smem + lay.stage_off + (warp - 4) * GEMM_EPI_TILE_BYTES;
+  } else if (warp >= 4 && warp < 4 + EPI_WARPS) {
+    // ===================== consumers: wgmma main loop, then the epilogue =====================
+    // The accumulators leave the registers into the shared-memory accumulator tile (32 x 32 int32 chunks, 128 B rows,
+    // 16 B units XOR-swizzled by row&7: conflict-free both ways); the epilogue reads each chunk in the transposed
+    // mapping: 8 lanes x 16 B = one full 128 B line per row, 4 rows per instruction, per-column parameters loaded once
+    // per thread per chunk.
+    const int cw = warp - 4;            // consumer warp 0..7
+    const int wg = cw >> 2;             // its warpgroup: accumulator rows [64 wg, 64 wg + 64)
+    const bool wg_leader = (threadIdx.x & 127) == 0;
+    const int q = cw & 3;               // epilogue: row quarter [32q, 32q + 32) of the tile
+    const int half = cw >> 2;           // which of the two warps sharing this row quarter
+    const int nch = (p.BN + 31) >> 5;   // 32-column chunks per row quarter of the accumulator tile
+    uint8_t* const acc_tile = smem + lay.stage_off;
+    const uint8_t* stg = acc_tile;
+    constexpr bool BF16 = MODE >= 0 && (MODE & EPI_BF16) != 0;
+    using AccT = typename std::conditional<BF16, float, uint32_t>::type;
+    int stage = 0;
+    uint32_t phase = 0;
     const int rsub = lane >> 3;   // row within a group of 4
     const int cq = lane & 7;      // column quad within the 32-column chunk
     constexpr bool QPRE = gemm_qpre(MODE);
@@ -562,8 +603,6 @@ gemm_i8_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     const float* const ep_scale = QPRE ? p.scale_q : p.scale;      // per-column epilogue constants of this mode
     const float* const ep_bias = QPRE ? p.bias_q : p.bias;
     const bool conv = MODE < 0 ? (p.taps == 9) : ((MODE & EPI_CONV) != 0);
-    int acc = 0;
-    uint32_t acc_phase = 0;
     // ---- residual ring (RES_TMA): work items of this warp = (tile, chunk) in processing order; `pf_*` is the prefetch
     // cursor, GEMM_RES_NBUF - 1 items ahead of the item being finalised
     uint8_t* rring = smem + lay.res_off + (warp - 4) * (GEMM_RES_NBUF * 4096);
@@ -589,7 +628,7 @@ gemm_i8_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     }
     for (int item = blockIdx.x; item < num_tiles; item += gridDim.x) {
       const int tile = item / splits;
-      [[maybe_unused]] const int zsplit = item - tile * splits;
+      const int zsplit = item - tile * splits;
       const int tm = tile / p.tiles_n;
       const int tn = tile - tm * p.tiles_n;
       const int n_base = tn * p.BN;
@@ -601,46 +640,88 @@ gemm_i8_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
 #pragma unroll
         for (int it = 0; it < 8; ++it) gemm_row_meta(p, m_warp + it * 4 + rsub, cls8[it], img8[it]);
       }
-      mbar_wait(&tmem_full[acc], acc_phase);
-      tc_fence_after();
-      const uint32_t t_row = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(acc * 256);
-      if constexpr (MODE >= 0 && (MODE & EPI_SPLITK) != 0) {
-        // raw accumulators of this K slice -> ws[zsplit][M][N], 16-byte stores through the staging tile (row-major, coalesced)
-        int32_t* wz = p.ws + (long long)zsplit * p.M * p.N;
-        for (int c = half * 32; c < p.BN; c += CSTEP) {
-          const int ncols = (p.BN - c) >= 32 ? 32 : 16;
-          if (ncols == 32) {
-            uint32_t v[32];
-            tmem_ld_32x32(t_row + (uint32_t)c, v);
-            tmem_ld_wait();
+      // ---- main loop: k-blocks [kb0, kb1) of this work item; a stage returns to the producer once the MMAs reading it
+      // are complete (one k-block of MMAs stays in flight).  The accumulators live in this scope only: dead during the
+      // epilogue, whose registers they would otherwise take.
+      {
+        AccT accr[NS][32];
 #pragma unroll
-            for (int j = 0; j < 8; ++j)
-              *reinterpret_cast<uint4*>(stg + lane * 128 + ((j ^ (lane & 7)) << 4)) =
-                  make_uint4(v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]);
-          } else {
-            uint32_t v[16];
-            tmem_ld_32x16(t_row + (uint32_t)c, v);
-            tmem_ld_wait();
+        for (int s = 0; s < NS; ++s)
 #pragma unroll
-            for (int j = 0; j < 4; ++j)
-              *reinterpret_cast<uint4*>(stg + lane * 128 + ((j ^ (lane & 7)) << 4)) =
-                  make_uint4(v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]);
+          for (int i = 0; i < 32; ++i) accr[s][i] = 0;
+        const int kb0 = zsplit * kb_slice;
+        const int kb1 = min(num_kb_all, kb0 + kb_slice);
+        int prev_stage = -1;
+        // the N-tile width and the operand signedness are selected once per work item; each configuration's k-loop is
+        // its own straight-line wgmma sequence
+        auto mainloop = [&](auto cfg) {
+          using Cfg = decltype(cfg);
+          for (int kb = kb0; kb < kb1; ++kb) {
+            mbar_wait(&full_bar[stage], phase);
+            if constexpr (W4) mbar_wait(&ready_bar[stage], phase);   // ... and the B tile has been unpacked
+            wgmma_fence();
+            const uint32_t sa = smem_u32(smem + (size_t)stage * lay.stage_bytes);
+            const uint64_t da = make_smem_desc_sw128(sa + (uint32_t)(wg * 64 * GEMM_BK));
+            const uint64_t db = make_smem_desc_sw128(sa + GEMM_A_STAGE_BYTES);
+            gemm_wgmma_kblock<BF16, Cfg::SIGNED, Cfg::NF, Cfg::TAIL>(accr, da, db, kb > kb0 ? 1u : 0u);
+            wgmma_commit();
+            wgmma_wait<1>();
+            if (prev_stage >= 0 && wg_leader) mbar_arrive(&empty_bar[prev_stage]);
+            prev_stage = stage;
+            if (++stage == p.stages) { stage = 0; phase ^= 1; }
           }
-          __syncwarp();
-          const int n = n_base + c + cq * 4;
-          if (cq * 4 < ncols && n < p.N) {
+          wgmma_wait<0>();
+        };
+        if constexpr (BF16) gemm_dispatch_bn<NS, true>(p.BN, mainloop);
+        else if (p.a_signed) gemm_dispatch_bn<NS, true>(p.BN, mainloop);
+        else gemm_dispatch_bn<NS, false>(p.BN, mainloop);
 #pragma unroll
-            for (int it = 0; it < 8; ++it) {
-              const int row = it * 4 + rsub;
-              const int m = m_warp + row;
-              if (m < p.M)
-                *reinterpret_cast<uint4*>(wz + (long long)m * p.N + n) =
-                    *reinterpret_cast<const uint4*>(stg + row * 128 + ((cq ^ (row & 7)) << 4));
+        for (int s = 0; s < NS; ++s) wgmma_fence_regs(accr[s]);
+        if (prev_stage >= 0 && wg_leader) mbar_arrive(&empty_bar[prev_stage]);
+        const int r0 = 64 * wg + 16 * (cw & 3) + (lane >> 2);
+        if constexpr (SPLITK) {
+          // raw accumulators of this K slice -> ws[zsplit][M][N] straight from the registers (host: N % 4 == 0); a warp
+          // store covers 8 rows x 32 contiguous bytes
+          int32_t* wz = p.ws + (long long)zsplit * p.M * p.N;
+#pragma unroll
+          for (int s = 0; s < NS; ++s)
+#pragma unroll
+            for (int j = 0; j < 8; ++j) {
+              const int n = n_base + 64 * s + 8 * j + 2 * (lane & 3);
+              if (64 * s + 8 * j < p.BN && n < p.N) {
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                  const int m = tm * GEMM_BM + r0 + 8 * h;
+                  if (m < p.M)
+                    *reinterpret_cast<uint2*>(wz + (long long)m * p.N + n) = make_uint2(accr[s][4 * j + 2 * h], accr[s][4 * j + 2 * h + 1]);
+                }
+              }
+            }
+          continue;
+        }
+        // ---- accumulators -> accumulator tile (after every consumer warp has finished reading the previous tile's)
+        named_bar_sync(1, EPI_WARPS * 32);
+#pragma unroll
+        for (int s = 0; s < NS; ++s)
+#pragma unroll
+          for (int j = 0; j < 8; ++j) {
+            const int col = 64 * s + 8 * j + 2 * (lane & 3);
+            if (col < p.BN) {
+#pragma unroll
+              for (int h = 0; h < 2; ++h) {
+                const int row = r0 + 8 * h;
+                uint8_t* dst = acc_tile + ((row >> 5) * nch + (col >> 5)) * GEMM_EPI_TILE_BYTES + (row & 31) * 128 +
+                               ((((col & 31) >> 2) ^ (row & 7)) << 4) + (col & 3) * 4;
+                uint32_t lo, hi;
+                if constexpr (BF16) { lo = __float_as_uint(accr[s][4 * j + 2 * h]); hi = __float_as_uint(accr[s][4 * j + 2 * h + 1]); }
+                else { lo = accr[s][4 * j + 2 * h]; hi = accr[s][4 * j + 2 * h + 1]; }
+                *reinterpret_cast<uint2*>(dst) = make_uint2(lo, hi);
+              }
             }
           }
-          __syncwarp();
-        }
-      } else if constexpr (kTrans) {
+      }
+      named_bar_sync(1, EPI_WARPS * 32);
+      if constexpr (kTrans) {
         // V^T code output [img][n][token'] (token' = att_vt_perm order inside each group of 16).  The warp's
         // 32 tokens x 32 channels go through the staging tile; each lane then owns ONE channel and emits whole
         // 16-token groups as 16 B stores (the thread-per-row form below needs 32 byte stores per lane and chunk).
@@ -649,24 +730,7 @@ gemm_i8_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         const int tok0 = m_warp - img * p.rows_per_batch;
         for (int c = half * 32; c < p.BN; c += CSTEP) {
           const int ncols = (p.BN - c) >= 32 ? 32 : 16;
-          if (ncols == 32) {
-            uint32_t v[32];
-            tmem_ld_32x32(t_row + (uint32_t)c, v);
-            tmem_ld_wait();
-#pragma unroll
-            for (int j = 0; j < 8; ++j)
-              *reinterpret_cast<uint4*>(stg + lane * 128 + ((j ^ (lane & 7)) << 4)) =
-                  make_uint4(v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]);
-          } else {
-            uint32_t v[16];
-            tmem_ld_32x16(t_row + (uint32_t)c, v);
-            tmem_ld_wait();
-#pragma unroll
-            for (int j = 0; j < 4; ++j)
-              *reinterpret_cast<uint4*>(stg + lane * 128 + ((j ^ (lane & 7)) << 4)) =
-                  make_uint4(v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]);
-          }
-          __syncwarp();
+          stg = acc_tile + (q * nch + (c >> 5)) * GEMM_EPI_TILE_BYTES;
           const int col = ncols == 32 ? lane : (lane & 15);
           const int n = n_base + c + col;
           if (m_warp < p.M && n < p.N) {
@@ -698,14 +762,7 @@ gemm_i8_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         // holds 4 x (4 x-features | 4 gate-features); lane -> (row group of 8, pair); 4 iterations cover 32 rows.
         const int r8 = lane >> 2, pq = lane & 3;
         for (int c = half * 32; c < p.BN; c += CSTEP) {
-          uint32_t v[32];
-          tmem_ld_32x32(t_row + (uint32_t)c, v);
-          tmem_ld_wait();
-#pragma unroll
-          for (int j = 0; j < 8; ++j)
-            *reinterpret_cast<uint4*>(stg + lane * 128 + ((j ^ (lane & 7)) << 4)) =
-                make_uint4(v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]);
-          __syncwarp();
+          stg = acc_tile + (q * nch + (c >> 5)) * GEMM_EPI_TILE_BYTES;
           const int nx = n_base + c + 8 * pq;          // 4 x columns, then 4 gate columns
           if (nx < p.N) {
             const float4 sx = __ldg(reinterpret_cast<const float4*>(p.scale + nx));
@@ -746,37 +803,18 @@ gemm_i8_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         for (int c = half * 32; c < p.BN; c += CSTEP) {
           if (p.BN - c >= 32) {
             uint32_t v[32];
-            tmem_ld_32x32(t_row + (uint32_t)c, v);
-            tmem_ld_wait();
+            gemm_acc_row(acc_tile + (q * nch + (c >> 5)) * GEMM_EPI_TILE_BYTES, lane, v);
             if (m < p.M && n_base + c < p.N) gemm_epilogue_rowwise<32>(p, qk, v, m, n_base + c, cls, img);
           } else {
             uint32_t v[16];
-            tmem_ld_32x16(t_row + (uint32_t)c, v);
-            tmem_ld_wait();
+            gemm_acc_row(acc_tile + (q * nch + (c >> 5)) * GEMM_EPI_TILE_BYTES, lane, v);
             if (m < p.M && n_base + c < p.N) gemm_epilogue_rowwise<16>(p, qk, v, m, n_base + c, cls, img);
           }
         }
       } else {
         for (int c = half * 32; c < p.BN; c += CSTEP) {
           const int ncols = (p.BN - c) >= 32 ? 32 : 16;
-          if (ncols == 32) {
-            uint32_t v[32];
-            tmem_ld_32x32(t_row + (uint32_t)c, v);
-            tmem_ld_wait();
-#pragma unroll
-            for (int j = 0; j < 8; ++j)
-              *reinterpret_cast<uint4*>(stg + lane * 128 + ((j ^ (lane & 7)) << 4)) =
-                  make_uint4(v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]);
-          } else {
-            uint32_t v[16];
-            tmem_ld_32x16(t_row + (uint32_t)c, v);
-            tmem_ld_wait();
-#pragma unroll
-            for (int j = 0; j < 4; ++j)
-              *reinterpret_cast<uint4*>(stg + lane * 128 + ((j ^ (lane & 7)) << 4)) =
-                  make_uint4(v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]);
-          }
-          __syncwarp();
+          stg = acc_tile + (q * nch + (c >> 5)) * GEMM_EPI_TILE_BYTES;
           const uint8_t* rbuf = nullptr;
           if constexpr (RES_TMA) {
             res_issue();                              // keep GEMM_RES_NBUF - 1 loads in flight
@@ -888,17 +926,8 @@ gemm_i8_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
           __syncwarp();
         }
       }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&tmem_empty[acc]);
-      if (++acc == 2) { acc = 0; acc_phase ^= 1; }
     }
   }
-
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  if (warp == 2) tmem_dealloc(tmem_base, 512);
 }
 
 // Second half of a split-K GEMM: sum the K slices (int32: exact in any order) and apply the fp32 epilogue of the plain

@@ -3,7 +3,7 @@
 //
 // The straightforward form rintf(__fdiv_rn(y, d)) + zp -> clamp -> (int) costs 4 XU-pipe operations per
 // element (FCHK, MUFU.RCP, FRND, F2I; the XU pipe runs at 16 lanes/clk/SM), which made the "memory-bound"
-// norm/quantise kernels XU-bound at ~15-25% of HBM bandwidth (profiles/r01_elementwise_xu.txt).  This
+// norm/quantise kernels XU-bound well below HBM bandwidth.  This
 // version uses no XU operation per element:
 //   * y/d as q0 = y*r, q = fma(fma(-q0, d, y), r, q0) with r = RN(1/d): one Newton step on the FMA pipe,
 //     correctly rounded except for vanishingly rare halfway cases;
@@ -90,8 +90,7 @@ __device__ __forceinline__ float silu_fast(float x) {
 // exact-erf GELU (F.gelu default, ldm/modules/attention.py:44)
 __device__ __forceinline__ float gelu_erf(float x) { return 0.5f * x * (1.0f + erff(x * 0.70710678118654752440f)); }
 
-// The same function in ~15 instructions (libm erff is ~40, which made the GEGLU GEMM epilogue issue-bound:
-// profiles/r01_gemm_smallk.txt).  erfc(z) = t*P(t)*exp(-z^2), t = 1/(1 + p z) (Abramowitz-Stegun 7.1.26) with
+// The same function in ~15 instructions (libm erff is ~40, which made the GEGLU GEMM epilogue issue-bound).  erfc(z) = t*P(t)*exp(-z^2), t = 1/(1 + p z) (Abramowitz-Stegun 7.1.26) with
 // the 1/2 and the 1/sqrt(2) folded into the constants, evaluated on the complementary side so that negative
 // gates lose no precision:  gelu(g) = g - h (g >= 0), -h (g < 0), h = |g| * erfc(|g|/sqrt2) / 2.
 // Max |error| 3.3e-7 over [-8, 8] in fp32 (torch's own fp32 F.gelu: 1.2e-6), measured in tools/check_gelu.py.

@@ -1,6 +1,6 @@
-"""qdiff_b200: B200-native drop-in for the `qdiff` package of Xiuyu-Li/q-diffusion (hot path only).
+"""qdiff_b200: H100-native (sm_90a) drop-in for the `qdiff` package of Xiuyu-Li/q-diffusion (hot path only).
 
-Exports mirror qdiff/__init__.py:1-5.  Compute lives in libqdiff_b200.so (sm_100a); importing this
+Exports mirror qdiff/__init__.py:1-5.  Compute lives in libqdiff_b200.so (sm_90a); importing this
 package does not need a GPU, running a UNet does.
 """
 from .adaptive_rounding import AdaRoundQuantizer

@@ -150,7 +150,7 @@ def lib():
     if not os.path.exists(LIB_PATH):
         raise RuntimeError(
             f"qdiff_b200: {LIB_PATH} is missing. Build it with `python __graft_entry__.py` "
-            "(nvcc, sm_100a). There is no CPU fallback.")
+            "(nvcc, sm_90a). There is no CPU fallback.")
     L = C.CDLL(LIB_PATH)
     for name in EXPORTS:
         getattr(L, name)  # raises AttributeError when a declared symbol is not exported

@@ -177,7 +177,7 @@ def _dist_env():
 def _setup(seed):
     import torch
     if not torch.cuda.is_available():
-        raise SystemExit("qdiff_b200 scripts need a CUDA device (sm_100a): the engine has no CPU fallback")
+        raise SystemExit("qdiff_b200 scripts need a CUDA device (sm_90a): the engine has no CPU fallback")
     rank, world, local = _dist_env()
     torch.cuda.set_device(local)
     if world > 1:

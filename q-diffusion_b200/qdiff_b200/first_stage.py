@@ -13,7 +13,7 @@ load_state_dict(strict=False).  `.decode()` lowers the graph once per latent sha
 replays it; there is no torch / CPU path.
 
 Arithmetic.  The first stage is NOT quantised by q-diffusion: weights and activations are floating point.  Every conv /
-1x1 conv is a tcgen05 kind::f16 contraction with fp32 accumulation (the same kernel as the weight-only UNet path) on
+1x1 conv is a bf16 wgmma contraction with fp32 accumulation (the same kernel as the weight-only UNet path) on
 bfloat16 PLANES of both operands: x = x_hi + x_mid + x_lo and w = w_hi + w_mid + w_lo, each plane a bfloat16 rounding of
 the remainder.  `precision` picks the plane products that are formed:
     1  x_hi w_hi                                            (plain bfloat16: relative 2^-9 per product)
@@ -324,7 +324,7 @@ class FirstStageBuilder(graph.WeightOnlyBuilder):
             self.add(_lib.QD_OP_GEMM, d, label + (f".pass{i}" if i else ""), flops=2 * M * N * Cp if i == 0 else 0)
 
     def attn_products_tc(self, q, k, v, T, C_, label):
-        """softmax(q k^T C^-1/2) v with both products as bfloat16-plane GEMMs on tcgen05 (fp32 accumulation), per image:
+        """softmax(q k^T C^-1/2) v with both products as bfloat16-plane GEMMs on wgmma (fp32 accumulation), per image:
         S = q k^T with all six plane products (the scores sit in an exponent: 2^-24), row softmax in fp32 (qd_softmax_rows),
         O = P v with the decoder's precision.  K and V^T are run-time operands: their weight tiles are copied from their own
         plane splits.  Replaces the fp32 CUDA-core kernel where it dominated the decode (SD: 26 %, bedroom: 58 %)."""

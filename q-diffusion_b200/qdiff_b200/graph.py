@@ -643,7 +643,7 @@ class Builder:
 
     @staticmethod
     def head_pitch(d):
-        """Per-head pitch of the Q/K code layout: the tcgen05 attention kernel wants d padded to the TMA swizzle span."""
+        """Per-head pitch of the Q/K code layout: d padded to 32 / 64 / 128 bytes (aligned rows for the attention kernels)."""
         return 32 if d <= 32 else 64 if d <= 64 else 128 if d <= 112 else d
 
     @staticmethod
@@ -1185,7 +1185,7 @@ class WeightOnlyBuilder(Builder):
     set_quant_state(False, False): the full-precision state the reference uses for FP baselines and calibration data.
 
     Every QuantModule becomes  y = delta_w[n] * sum_k x[m,k] * ws[n,k] + bias  with the fp32 activation split into three
-    bfloat16 planes (qd_split_bf16x3) and the integer weight codes held exactly in bfloat16: a tcgen05 kind::f16
+    bfloat16 planes (qd_split_bf16x3) and the integer weight codes held exactly in bfloat16: a bf16 wgmma
     contraction with fp32 accumulation, i.e. the reference's fp32 conv up to summation order.  With use_weight_quant
     False the fp32 weight is split into three bfloat16 planes as well and the six plane products down to 2^-24 are formed
     in three accumulating launches (x_{hi,mid,lo} w_hi, x_{hi,mid} w_mid, x_hi w_lo: qd_gemm_desc.lda = plane pitch).

@@ -128,7 +128,7 @@ class QuantModule(nn.Module):
 
     Holds the FP weight/bias (shared Parameters), the weight and activation quantizers (plus the
     `_0` pair after `set_split`, split-shortcut) and the state flags.  The layer itself executes as
-    an INT8 tcgen05 GEMM inside the engine program; calling `forward` on a single wrapped layer is
+    an INT8 wgmma GEMM inside the engine program; calling `forward` on a single wrapped layer is
     not part of the sampling path and is not provided.
     """
 

@@ -1,7 +1,7 @@
 """Host-side mirror of qdiff/quant_model.py -- the drop-in API boundary (reference :12-97).
 
 Quantisation states the engine realises (set_quant_state, reference :52-55):
-    (True, True)   weights and activations quantised (W4A8 / W8A8): INT8 tcgen05 GEMMs, all four UNet configurations;
+    (True, True)   weights and activations quantised (W4A8 / W8A8): INT8 wgmma GEMMs, all four UNet configurations;
     (True, False)  weight-only (what resume_cali_model(..., quant_act=False) leaves, qdiff/utils.py:407): fp32 activations
                    as bfloat16 x3 planes against exact bfloat16 weight codes, fp32 accumulation; DDIM (CIFAR) family;
     (False, False) full precision: NOT realised (it is the reference's own path for FP baselines / calibration data).

@@ -1,7 +1,7 @@
 """First-stage decode on the engine vs the oracle and the reference's committed outputs (SURVEY section 8 row f2).
 
 The first stage is floating point (not quantised by q-diffusion), so the bar is a stated tolerance: the engine contracts
-bfloat16 planes of both operands on tcgen05 with fp32 accumulation; `precision` = plane products per MAC (1, 3 or 6).
+bfloat16 planes of both operands on wgmma with fp32 accumulation; `precision` = plane products per MAC (1, 3 or 6).
 Tolerances (relative to max |reference|), calibrated by emulating the plane arithmetic in float64 on the two fixtures
 (1: 0.7-1.5e-2, 3: 1.6-3.7e-5, 6: 0.6-1.4e-6) with headroom for fp32 accumulation order."""
 import os

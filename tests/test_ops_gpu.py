@@ -556,7 +556,7 @@ def test_qattention(cuda, B, heads, d, Tq, Tk, sym, sm_bits):
     (2, 2, 16, 160, 160, False, 16),   # 32-byte rows
 ])
 def test_qattention_f16_operands(cuda, B, heads, d, Tq, Tk, sym, sm_bits):
-    """qd_attention_desc.qk_f16: Q / K as fp16 centred codes, QK^T on tcgen05 kind::f16 - the same integers as the code path,
+    """qd_attention_desc.qk_f16: Q / K as fp16 centred codes, QK^T on f16 MMAs (fp32 accumulation) - the same integers as the code path,
     so the result must agree with the fake-quant oracle to the same tolerance AND with the code path closely."""
     out, ref = _run_attention(cuda, B, heads, d, Tq, Tk, sym, sm_bits, seed=B * 1000 + d, f16=True)
     base, _ = _run_attention(cuda, B, heads, d, Tq, Tk, sym, sm_bits, seed=B * 1000 + d, f16=False)

@@ -1,4 +1,4 @@
-"""Micro-benchmark of the INT8 tcgen05 GEMM / conv kernel on the SD v1-4 UNet layer shapes
+"""Micro-benchmark of the INT8 wgmma GEMM / conv kernel on the SD v1-4 UNet layer shapes
 (SURVEY Appendix B), batch 16 (8 images x CFG).  Prints achieved TOP/s per shape.
 Usage: python tools/bench_gemm.py [--iters 20]"""
 import argparse

@@ -16,7 +16,7 @@ T = int(sys.argv[1]) if len(sys.argv) > 1 else 4096
 Tk = int(sys.argv[2]) if len(sys.argv) > 2 else T
 Tkp = (Tk + 15) // 16 * 16
 P = 64
-F16 = os.environ.get("ATTN_F16", "1") != "0"      # Q / K as fp16 centred codes (qd_attention_desc.qk_f16), the engine's default
+F16 = os.environ.get("ATTN_F16", "1") != "0"      # Q / K as fp16 centred codes (qd_attention_desc.qk_f16), the engine's default for d <= 64
 if F16:
     P = 128
     q = torch.zeros(B, T, heads, P // 2, dtype=torch.float16, device=dev)

@@ -1,8 +1,8 @@
 """smoke(): ONE small invocation of the hot path on cuda:0, checked against the CPU oracle.
 
 Order matters for the driver's launch trace (it records the first ~1000 kernel launches): the hand-written kernels run
-FIRST, called directly through the C ABI (INT8 tcgen05 GEMM, implicit-GEMM conv3x3, GEGLU epilogue, tcgen05 / small-Tk /
-mma.sync attention, GroupNorm, LayerNorm, quantizer) and checked against the op oracle; only then the SD-style tiny UNet
+FIRST, called directly through the C ABI (INT8 wgmma GEMM, implicit-GEMM conv3x3, GEGLU epilogue, small-Tk / mma.sync
+attention, GroupNorm, LayerNorm, quantizer) and checked against the op oracle; only then the SD-style tiny UNet
 fixture (spatial transformer + cross attention, asymmetric W4A8, sm_abit 16, split shortcut) is folded (torch ops on
 the GPU: load-time only) and run through QuantModel.forward and two PLMS steps of the sampler."""
 import torch

@@ -26,7 +26,7 @@ SHAPES = [
     ("lin 2560->640 @1024 f32res", 16, 32, 32, 2560, 640, 1, "f32res"),
     ("lin 1280->1280 @256 q", 16, 16, 16, 1280, 1280, 1, "q"),
 ]
-BNS = [0, 64, 80, 96, 112, 128, 160, 192, 224, 256]
+BNS = [0, 64, 80, 96, 112, 128]            # forced widths: plan_gemm takes bn_hint <= 128
 # --small: the short-M convs of the deep UNet levels (church 4x4 / 8x8 at batch 32 with 8-bit weights = doubled K axis;
 # SD 8x8 / 16x16 at batch 16): few M tiles, long K - the N tile decides how many SMs share the K loop
 SMALL = [
@@ -39,7 +39,7 @@ SMALL = [
     ("sd conv 2560->1280 @8", 16, 8, 8, 2560, 1280, 9, "f32", 1),
     ("sd conv 2560->1280 @16", 16, 16, 16, 2560, 1280, 9, "f32", 1),
 ]
-SMALL_BNS = [0, 16, 32, 48, 64, 80, 96, 128, 160, 192, 256]
+SMALL_BNS = [0, 16, 32, 48, 64, 80, 96, 128]
 
 
 def main():
