@@ -363,6 +363,30 @@ typedef struct qd_sampler_desc {
 int qd_sampler_step(const qd_sampler_desc* d, qd_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------
+ * qd_ancestral_step -- the ancestral DDPM update: posterior mean of (x0, x_t) plus scaled noise.
+ *   ddpm_steps of the CIFAR script        ddim/functions/denoising.py:53-65  (x0 clamped, sigma = sqrt(beta_t))
+ *   LatentDiffusion p_sample (-v)         ldm/models/diffusion/ddpm.py:220-233, 1052-1112
+ *                                         (predict_start_from_noise + q_posterior, no clamp, sigma = exp(0.5 logvar))
+ *   x0 = c_x * x - c_e * eps;  if (clamp) x0 = clamp(x0, -1, 1)
+ *   x_prev = m_x0 * x0 + m_x * x + sigma * noise          (no noise term when noise == NULL, e.g. t == 0)
+ * All tensors fp32, n elements each.
+ * ------------------------------------------------------------------------------------------ */
+typedef struct qd_ancestral_desc {
+  const float* x;
+  const float* eps;
+  const float* noise;     /* NULL: no noise term */
+  float* x_prev;
+  float* pred_x0;         /* optional: the (clamped) x0 */
+  long long n;
+  float c_x, c_e;
+  float m_x0, m_x;
+  float sigma;
+  int32_t clamp;
+} qd_ancestral_desc;
+
+int qd_ancestral_step(const qd_ancestral_desc* d, qd_stream_t stream);
+
+/* ------------------------------------------------------------------------------------------
  * Engine: a recorded program of the ops above for one UNet (QuantModel.forward,
  * qdiff/quant_model.py:68-69 -> UNetModel.forward openaimodel.py:745-782 / Model.forward
  * ddim/models/diffusion.py:308-360).  The host graph builder (qdiff_b200/graph.py) records ops

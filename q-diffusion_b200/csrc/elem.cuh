@@ -910,4 +910,19 @@ __global__ void sampler_step_kernel(const qd_sampler_desc p) {
   }
 }
 
+// Ancestral (posterior-mean) update: x0 = c_x x - c_e eps, optionally clamped to [-1, 1] (NaN passes through like
+// torch.clamp), x_prev = m_x0 x0 + m_x x + sigma noise.
+__global__ void ancestral_step_kernel(const qd_ancestral_desc p) {
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < p.n;
+       i += (long long)gridDim.x * blockDim.x) {
+    const float x = p.x[i];
+    float x0 = p.c_x * x - p.c_e * p.eps[i];
+    if (p.clamp) x0 = x0 < -1.f ? -1.f : (x0 > 1.f ? 1.f : x0);
+    float xp = p.m_x0 * x0 + p.m_x * x;
+    if (p.noise) xp += p.sigma * p.noise[i];
+    if (p.pred_x0) p.pred_x0[i] = x0;
+    p.x_prev[i] = xp;
+  }
+}
+
 }  // namespace qd

@@ -1005,6 +1005,11 @@ int qd_sampler_step(const qd_sampler_desc* d, qd_stream_t s) {
   launch_k(qd::sampler_step_kernel, grid_for(d->n, 256), 256, 0, (cudaStream_t)s, *d);
   return check_launch("sampler_step_kernel");
 }
+int qd_ancestral_step(const qd_ancestral_desc* d, qd_stream_t s) {
+  if (!d || !d->x || !d->eps || !d->x_prev || d->n <= 0) return fail(QD_ERR_BAD_ARG, "ancestral: bad args");
+  launch_k(qd::ancestral_step_kernel, grid_for(d->n, 256), 256, 0, (cudaStream_t)s, *d);
+  return check_launch("ancestral_step_kernel");
+}
 
 int qd_engine_create(int device, qd_engine** out) {
   if (!out) return fail(QD_ERR_BAD_ARG, "null out");

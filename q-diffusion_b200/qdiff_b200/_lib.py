@@ -132,10 +132,17 @@ class SamplerDesc(C.Structure):
     ]
 
 
+class AncestralDesc(C.Structure):
+    _fields_ = [
+        ("x", c_vp), ("eps", c_vp), ("noise", c_vp), ("x_prev", c_vp), ("pred_x0", c_vp),
+        ("n", c_ll), ("c_x", c_f), ("c_e", c_f), ("m_x0", c_f), ("m_x", c_f), ("sigma", c_f), ("clamp", c_i32),
+    ]
+
+
 EXPORTS = [
     "qd_qgemm_i8", "qd_quantize", "qd_groupnorm_quant", "qd_groupnorm_workspace_floats", "qd_layernorm_quant",
     "qd_im2col_i8", "qd_qattention", "qd_split_bf16x3", "qd_attention_fp32", "qd_lincomb3", "qd_timestep_embedding", "qd_copy2d", "qd_nchw_to_nhwc", "qd_nhwc_to_nchw", "qd_avgpool2x", "qd_upsample2x_f32", "qd_vq_lookup", "qd_softmax_rows",
-    "qd_sampler_step", "qd_engine_create", "qd_engine_add_op", "qd_engine_num_ops", "qd_engine_finalize",
+    "qd_sampler_step", "qd_ancestral_step", "qd_engine_create", "qd_engine_add_op", "qd_engine_num_ops", "qd_engine_finalize",
     "qd_engine_run", "qd_engine_run_range", "qd_engine_destroy", "qd_last_error", "qd_num_sms", "qd_launch_count",
 ]
 
@@ -157,7 +164,7 @@ def lib():
     L.qd_last_error.restype = C.c_char_p
     L.qd_launch_count.restype = c_ll
     for name in ("qd_qgemm_i8", "qd_quantize", "qd_groupnorm_quant", "qd_layernorm_quant", "qd_im2col_i8",
-                 "qd_qattention", "qd_sampler_step", "qd_split_bf16x3", "qd_attention_fp32"):
+                 "qd_qattention", "qd_sampler_step", "qd_ancestral_step", "qd_split_bf16x3", "qd_attention_fp32"):
         getattr(L, name).argtypes = [c_vp, c_vp]
         getattr(L, name).restype = C.c_int
     L.qd_timestep_embedding.argtypes = [c_vp, c_vp, c_i32, c_i32, c_i32, c_vp, c_vp]

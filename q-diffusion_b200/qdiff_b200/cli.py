@@ -4,7 +4,10 @@
     scripts/sample_diffusion_ldm.py    <- reference scripts/sample_diffusion_ldm.py:191-349    (unconditional LDM)
     scripts/txt2img.py                 <- reference scripts/txt2img.py:107-331                 (Stable Diffusion)
 
-Same flags, same meaning; what runs underneath is the engine.  Scope (SURVEY section 8): the denoising loop on a
+Same flags, same meaning; what runs underneath is the engine.  Samplers: sample_diffusion_ddim.py --sample_type
+generalized (DDIM), ddpm_noisy (ancestral DDPM) and dpm_solver (singlestep DPM-Solver++, order 3); sample_diffusion_ldm.py
+DDIM (default), --dpm (DPM-Solver++ 2M) and -v (the 1000-step ancestral loop); txt2img.py DDIM and --plms.  The saved meta
+names the sampler and its NFE (UNet calls per image batch).  Scope (SURVEY section 8): the denoising loop on a
 calibrated checkpoint -- `--ptq --resume --cali_ckpt ckpt.pth` (the checkpoint the reference's calibration wrote; it
 carries the FP weights, the AdaRound parameters and the activation quantizers, SURVEY Appendix C, so no base checkpoint
 is needed).  Calibration itself (`--ptq` without `--resume`), `--resume_w` and the text encoder
@@ -288,6 +291,17 @@ def _decode_images(fs, scale_factor, z, dev, chunk=4):
     return torch.cat(outs)
 
 
+class _CountingModel:
+    """The eps-model callable handed to a sampler loop, counting its calls (the NFE recorded in the saved meta)."""
+
+    def __init__(self, fn):
+        self.fn, self.calls = fn, 0
+
+    def __call__(self, *a):
+        self.calls += 1
+        return self.fn(*a)
+
+
 def _shard(n_total, world):
     if n_total % world:
         raise SystemExit(f"batch size {n_total} is not divisible by the {world} ranks")
@@ -296,7 +310,13 @@ def _shard(n_total, world):
 
 # ---------------------------------------------------------------------------------------------- sample_diffusion_ddim
 def run_ddim(args):
-    """Diffusion.sample / sample_fid / sample_image of the reference script (:110-347) on the engine."""
+    """Diffusion.sample / sample_fid / sample_image of the reference script (:110-347) on the engine.  --sample_type:
+    generalized -> samplers.generalized_steps; ddpm_noisy -> samplers.ddpm_steps (honours --skip_type; the reference's
+    branch imports `functions.denoising`, a module path that does not exist (SURVEY Appendix D Q10), so it never runs
+    there -- the engine implements the function that path names, ddim/functions/denoising.py:ddpm_steps);
+    dpm_solver -> samplers.dpm_solver_singlestep with --timesteps as the NFE (--skip_type / --eta are not used, as in the
+    reference); anything else raises NotImplementedError like the reference.  Stochastic steps draw the full-batch noise
+    per step from the round's seed and keep this rank's slice (dist.step_noise_fn)."""
     import numpy as np
     import torch
     from . import dist as qdist, samplers, unet
@@ -326,33 +346,46 @@ def run_ddim(args):
         raise SystemExit("only the linear beta schedule of the reference's configs is supported")
     T = d["num_diffusion_timesteps"]
     betas = torch.from_numpy(np.linspace(d["beta_start"], d["beta_end"], T, dtype=np.float64)).float()
-    if args.sample_type != "generalized":
-        raise SystemExit(f"--sample_type {args.sample_type}: the engine implements 'generalized' (DDIM); DPM-Solver / "
-                         "ddpm_noisy are listed under SURVEY section 8 f3")
-    if args.skip_type == "uniform":
-        seq = list(range(0, T, T // args.timesteps))
-    elif args.skip_type == "quad":
-        seq = [int(s) for s in list(np.linspace(0, np.sqrt(T * 0.8), args.timesteps) ** 2)]
-    else:
-        raise NotImplementedError(args.skip_type)
+    kind = args.sample_type
+    if kind not in ("generalized", "ddpm_noisy", "dpm_solver"):
+        raise NotImplementedError(kind)
+    seq = None
+    if kind != "dpm_solver":            # DPM-Solver: --timesteps is the NFE; --skip_type / --eta are not used
+        if args.skip_type == "uniform":
+            seq = list(range(0, T, T // args.timesteps))
+        elif args.skip_type == "quad":
+            seq = [int(s) for s in list(np.linspace(0, np.sqrt(T * 0.8), args.timesteps) ** 2)]
+        else:
+            raise NotImplementedError(args.skip_type)
     per = _shard(batch, world)
     n_rounds = max(1, -(-args.max_images // batch))
+    model = _CountingModel(lambda xx, tt: qnn(xx, tt))
     outs, t0 = [], time.time()
     for r in range(n_rounds):
         (x,) = qdist.shard_like_single_process((batch, ch, size, size), args.seed + r, rank, world)
-        noise_gen = torch.Generator().manual_seed(args.seed + 7919 * (r + 1))
-        full_noise = [torch.randn(batch, ch, size, size, generator=noise_gen) for _ in seq] if args.eta > 0 else None
+        noise_seed = args.seed + 7919 * (r + 1)
         lo = rank * per
-        x = samplers.generalized_steps(x.to(dev), seq, lambda xx, tt: qnn(xx, tt), betas, eta=args.eta,
-                                       noise_fn=(lambda k, shape, d_: full_noise[k][lo:lo + per].to(d_)) if full_noise else None)
+        if kind == "generalized":
+            noise_gen = torch.Generator().manual_seed(noise_seed)
+            full_noise = [torch.randn(batch, ch, size, size, generator=noise_gen) for _ in seq] if args.eta > 0 else None
+            x = samplers.generalized_steps(x.to(dev), seq, model, betas, eta=args.eta,
+                                           noise_fn=(lambda k, shape, d_: full_noise[k][lo:lo + per].to(d_)) if full_noise else None)
+        elif kind == "ddpm_noisy":
+            x = samplers.ddpm_steps(x.to(dev), seq, model, betas,
+                                    noise_fn=qdist.step_noise_fn((batch, ch, size, size), noise_seed, rank, world))
+        else:
+            x = samplers.dpm_solver_singlestep(x.to(dev), model, betas, steps=args.timesteps, order=3)
         x = qdist.gather_latents(x, world)
         outs.append(torch.clamp((x + 1.0) / 2.0, 0.0, 1.0))       # inverse_data_transform (rescaled data)
     imgs = torch.cat(outs)[:args.max_images]
     torch.cuda.synchronize()
     dt = time.time() - t0
+    nfe = model.calls // n_rounds
     if rank == 0:
-        print(f"{imgs.shape[0]} images, {len(seq)} steps each, {dt:.2f} s -> {imgs.shape[0] / dt:.2f} images/s on {world} GPU(s)")
-    return _save(args, args.logdir if args.logdir != "none" else ".", imgs, dict(kind="images", steps=len(seq)), rank)
+        print(f"{imgs.shape[0]} images, {kind} sampler, {nfe} UNet calls each, {dt:.2f} s -> {imgs.shape[0] / dt:.2f} "
+              f"images/s on {world} GPU(s)")
+    meta = dict(kind="images", steps=len(seq) if seq is not None else args.timesteps, sampler=kind, nfe=nfe)
+    return _save(args, args.logdir if args.logdir != "none" else ".", imgs, meta, rank)
 
 
 # ---------------------------------------------------------------------------------------------- sample_diffusion_ldm
@@ -369,15 +402,14 @@ def _ldm_config(args):
 
 
 def run_ldm(args):
-    """run / make_convolutional_sample / convsample_ddim of the reference script (:85-163) on the engine.  Saves the
-    LATENTS; with --b200_decode also the images, decoded by the first stage on the engine (qdiff_b200.first_stage)."""
+    """run / make_convolutional_sample / convsample_ddim of the reference script (:85-163) on the engine.  -v runs the
+    ancestral loop over all the config's timesteps (samplers.AncestralSampler; -c / -e are ignored, as in the reference),
+    --dpm DPM-Solver++, otherwise DDIM.  Saves the LATENTS; with --b200_decode also the images, decoded by the first
+    stage on the engine (qdiff_b200.first_stage)."""
     import torch
     from . import dist as qdist, samplers, unet
     _require_resume(args)
     rank, world, dev = _setup(args.seed)
-    if args.vanilla_sample:
-        raise SystemExit("the engine implements DDIM (default) and DPM-Solver++ (--dpm) sampling for this script, not the "
-                         "1000-step ancestral DDPM loop")
     if args.b200_synthetic:
         qnn, spec = _synthetic(args, "ldm")
         ch, size = spec["in_shape"][0], spec["in_shape"][1]
@@ -391,7 +423,13 @@ def run_ldm(args):
         sched = dict(timesteps=cfg.get("timesteps", 1000), linear_start=cfg.get("linear_start", 1e-4),
                      linear_end=cfg.get("linear_end", 2e-2))
     schedule = samplers.Schedule("linear", sched["timesteps"], sched["linear_start"], sched["linear_end"])
-    sampler = (samplers.DPMSolverSampler if args.dpm else samplers.DDIMSampler)(qnn, schedule)
+    model = _CountingModel(qnn)
+    if args.vanilla_sample:     # convsample(make_prog_row=True) -> progressive_denoising (sample_diffusion_ldm.py:67-80)
+        sampler, kind = samplers.AncestralSampler(model, schedule), "ancestral"
+    elif args.dpm:
+        sampler, kind = samplers.DPMSolverSampler(model, schedule), "dpm_solver"
+    else:
+        sampler, kind = samplers.DDIMSampler(model, schedule), "ddim"
     per = _shard(args.batch_size, world)
     outs, t0, r = [], time.time(), 0
     while sum(o.shape[0] for o in outs) < args.n_samples:
@@ -401,7 +439,11 @@ def run_ldm(args):
 
         def noise_fn(i, shape, d_, gen=gen, lo=lo):
             return torch.randn(args.batch_size, ch, size, size, generator=gen)[lo:lo + per].to(d_)
-        if args.dpm:      # convsample_dpm (sample_diffusion_ldm.py:96-103): deterministic, eta is not used
+        if args.vanilla_sample:   # all config timesteps; -c / -e are not used (as in the reference)
+            z, _ = sampler.sample(batch_size=per, shape=(ch, size, size), x_T=x_T,
+                                  noise_fn=qdist.step_noise_fn((args.batch_size, ch, size, size), args.seed + 7919 * (r + 1),
+                                                               rank, world))
+        elif args.dpm:    # convsample_dpm (sample_diffusion_ldm.py:96-103): deterministic, eta is not used
             z, _ = sampler.sample(S=args.custom_steps, batch_size=per, shape=(ch, size, size), x_T=x_T)
         else:
             z, _ = sampler.sample(S=args.custom_steps, batch_size=per, shape=(ch, size, size), eta=args.eta, x_T=x_T,
@@ -411,9 +453,11 @@ def run_ldm(args):
     z = torch.cat(outs)[:args.n_samples]
     torch.cuda.synchronize()
     dt = time.time() - t0
+    nfe = model.calls // r
     if rank == 0:
-        print(f"{z.shape[0]} latents, {args.custom_steps} DDIM steps (eta {args.eta}), {dt:.2f} s -> {z.shape[0] / dt:.2f} /s on {world} GPU(s)")
-    meta = dict(kind="latents", steps=args.custom_steps, eta=args.eta)
+        print(f"{z.shape[0]} latents, {kind} sampler, {nfe} UNet calls each, {dt:.2f} s -> {z.shape[0] / dt:.2f} /s on "
+              f"{world} GPU(s)")
+    meta = dict(kind="latents", steps=nfe if args.vanilla_sample else args.custom_steps, eta=args.eta, sampler=kind, nfe=nfe)
     if args.b200_decode and rank == 0:
         fs, sf = _first_stage(args, args.b200_synthetic, None if args.b200_synthetic else cfg, dev)
         t1 = time.time()

@@ -27,6 +27,19 @@ def shard_like_single_process(shape, seed, rank, world, extra_shapes=()):
     return out
 
 
+def step_noise_fn(shape, seed, rank, world):
+    """noise_fn(k, size, device) for the stochastic samplers: every call draws the next FULL-batch noise tensor from one
+    CPU generator seeded with `seed` and returns this rank's slice on `device`.  One step's noise is drawn when the step
+    needs it, so nothing is precomputed for the whole loop (1000 steps of CIFAR batch 64 would be ~0.8 GB).
+    shape[0] is the GLOBAL batch."""
+    g = torch.Generator().manual_seed(seed)
+    lo, hi = shard_bounds(shape[0], rank, world)
+
+    def noise_fn(k, size, device):
+        return torch.randn(tuple(shape), generator=g)[lo:hi].to(device)
+    return noise_fn
+
+
 def gather_latents(local, world):
     """Final image gather: all_gather of the per-rank latents, concatenated in rank order (rank 0 saves)."""
     if world == 1:

@@ -211,6 +211,10 @@ def sampler_step(desc):
     check(lib().qd_sampler_step(C.byref(desc), stream_ptr()), "qd_sampler_step")
 
 
+def ancestral_step(desc):
+    check(lib().qd_ancestral_step(C.byref(desc), stream_ptr()), "qd_ancestral_step")
+
+
 def lincomb3(out, a, x, b=0.0, y=None, c=0.0, z=None):
     check(lib().qd_lincomb3(ptr(out), float(a), ptr(x), float(b), ptr(y), float(c), ptr(z), x.numel(), stream_ptr()),
           "qd_lincomb3")

@@ -6,9 +6,13 @@ PLMS multistep weights, x0 prediction, x_{t-1}) per step; nothing leaves the dev
 
 Restates, with the same argument names:
   generalized_steps                     ddim/functions/denoising.py:10-32
+  ddpm_steps                            ddim/functions/denoising.py:35-67             (qd_ancestral_step)
   DDIMSampler.sample / p_sample_ddim    ldm/models/diffusion/ddim.py:57-220
   PLMSSampler.sample / p_sample_plms    ldm/models/diffusion/plms.py:58-240
-  schedules                             ldm/modules/diffusionmodules/util.py:21-74, ddpm.py:118-146
+  DPMSolverSampler.sample               ldm/models/diffusion/dpm_solver/sampler.py:24-82   (multistep, LDM --dpm)
+  dpm_solver_singlestep                 ddim/dpm_solver_pytorch.py:490-760, 1222-1240 (singlestep order 3, CIFAR)
+  AncestralSampler.sample               ldm/models/diffusion/ddpm.py:1052-1168        (progressive_denoising, -v)
+  schedules                             ldm/modules/diffusionmodules/util.py:21-74, ddpm.py:118-158
 """
 import math
 import os
@@ -17,7 +21,7 @@ import numpy as np
 import torch
 
 from . import ops
-from ._lib import SamplerDesc, ptr
+from ._lib import AncestralDesc, SamplerDesc, ptr
 
 
 # ------------------------------------------------------------------------------- schedules
@@ -30,15 +34,25 @@ def make_beta_schedule(schedule="linear", n_timestep=1000, linear_start=1e-4, li
 
 
 class Schedule:
-    """The buffers LatentDiffusion.register_schedule creates (ddpm.py:118-146), fp32 like the reference."""
+    """The buffers LatentDiffusion.register_schedule creates (ddpm.py:118-158, v_posterior = 0): computed in float64
+    numpy, stored fp32 like the reference's to_torch."""
 
     def __init__(self, beta_schedule="linear", timesteps=1000, linear_start=1e-4, linear_end=2e-2):
         betas = make_beta_schedule(beta_schedule, timesteps, linear_start, linear_end)
         ac = np.cumprod(1.0 - betas, axis=0)
+        ac_prev = np.append(1.0, ac[:-1])
+        f32 = lambda v: torch.tensor(v, dtype=torch.float32)    # noqa: E731
         self.num_timesteps = int(timesteps)
-        self.betas = torch.tensor(betas, dtype=torch.float32)
-        self.alphas_cumprod = torch.tensor(ac, dtype=torch.float32)
-        self.alphas_cumprod_prev = torch.tensor(np.append(1.0, ac[:-1]), dtype=torch.float32)
+        self.betas = f32(betas)
+        self.alphas_cumprod = f32(ac)
+        self.alphas_cumprod_prev = f32(ac_prev)
+        # what the ancestral loop reads (p_mean_variance: predict_start_from_noise + q_posterior)
+        self.sqrt_recip_alphas_cumprod = f32(np.sqrt(1. / ac))
+        self.sqrt_recipm1_alphas_cumprod = f32(np.sqrt(1. / ac - 1))
+        posterior_variance = betas * (1. - ac_prev) / (1. - ac)
+        self.posterior_log_variance_clipped = f32(np.log(np.maximum(posterior_variance, 1e-20)))
+        self.posterior_mean_coef1 = f32(betas * np.sqrt(ac_prev) / (1. - ac))
+        self.posterior_mean_coef2 = f32((1. - ac_prev) * np.sqrt(1. - betas) / (1. - ac))
 
 
 def make_ddim_timesteps(ddim_discr_method, num_ddim_timesteps, num_ddpm_timesteps):
@@ -80,6 +94,16 @@ def _step(x, eps, x_prev, *, a_t, a_prev, sigma, sqrt_one_minus_at=None, cfg_sca
     d.dir_coef = math.sqrt(max(1.0 - float(a_prev) - float(sigma) ** 2, 0.0))
     d.sigma = float(sigma)
     ops.sampler_step(d)
+
+
+def _ancestral(x, eps, x_prev, *, c_x, c_e, m_x0, m_x, sigma=0.0, noise=None, clamp=False, pred_x0=None):
+    d = AncestralDesc()
+    d.x, d.eps, d.x_prev = ptr(x), ptr(eps), ptr(x_prev)
+    d.noise, d.pred_x0 = ptr(noise), ptr(pred_x0)
+    d.n = x.numel()
+    d.c_x, d.c_e, d.m_x0, d.m_x, d.sigma = float(c_x), float(c_e), float(m_x0), float(m_x), float(sigma)
+    d.clamp = int(bool(clamp))
+    ops.ancestral_step(d)
 
 
 class _LatentSampler:
@@ -287,5 +311,178 @@ def generalized_steps(x, seq, model, b, eta=0.0, noise_fn=None):
         if c1 != 0.0:
             noise = noise_fn(k, tuple(x.shape), dev) if noise_fn is not None else torch.randn_like(cur)
         _step(cur, et, nxt, a_t=at, a_prev=at_next, sigma=c1, noise=noise)
+        cur, nxt = nxt, cur
+    return cur
+
+
+# ------------------------------------------------------------------------------- ancestral DDPM
+@torch.no_grad()
+def ddpm_steps(x, seq, model, b, noise_fn=None):
+    """Ancestral DDPM loop of the CIFAR script's `--sample_type ddpm_noisy` (ddim/functions/denoising.py:35-67).  Per step
+    one UNet call at the float timestep and one fused qd_ancestral_step: x0 = sqrt(1/at) x - sqrt(1/at - 1) e clamped to
+    [-1, 1], mean = (sqrt(atm1) beta_t x0 + sqrt(1 - beta_t) (1 - atm1) x) / (1 - at) with the division folded into the two
+    coefficients, noise scale exp(0.5 log beta_t) (beta_t = 1 - at / atm1, not the posterior variance), none at t == 0.
+    noise_fn(k, shape, device) supplies the draw of step k.  Returns the final x (device resident)."""
+    n = x.size(0)
+    dev = x.device
+    beta = torch.cat([torch.zeros(1), b.detach().cpu().float()], dim=0)
+    acp = (1 - beta).cumprod(dim=0)  # compute_alpha: index t+1
+    seq = list(seq)
+    seq_next = [-1] + seq[:-1]
+    cur, nxt = x.to(torch.float32).clone(), torch.empty_like(x, dtype=torch.float32)
+    for k, (i, j) in enumerate(zip(reversed(seq), reversed(seq_next))):
+        t = (torch.ones(n) * i).to(dev)
+        at, atm1 = acp[int(i) + 1], acp[int(j) + 1]
+        beta_t = 1 - at / atm1
+        et = model(cur, t.float())
+        noise = None
+        if i != 0:
+            noise = noise_fn(k, tuple(x.shape), dev) if noise_fn is not None else torch.randn_like(cur)
+        _ancestral(cur, et, nxt, c_x=(1.0 / at).sqrt(), c_e=(1.0 / at - 1).sqrt(),
+                   m_x0=atm1.sqrt() * beta_t / (1.0 - at), m_x=(1 - beta_t).sqrt() * (1 - atm1) / (1.0 - at),
+                   sigma=torch.exp(0.5 * beta_t.log()), noise=noise, clamp=True)
+        cur, nxt = nxt, cur
+    return cur
+
+
+class AncestralSampler(_LatentSampler):
+    """LatentDiffusion.progressive_denoising + p_sample + p_mean_variance (ldm/models/diffusion/ddpm.py:1052-1168), what
+    `sample_diffusion_ldm.py -v` runs (scripts/sample_diffusion_ldm.py:67-80, 115-117): timesteps num_timesteps-1 .. 0,
+    x_recon = predict_start_from_noise (NOT clamped: LatentDiffusion sets clip_denoised = False, ddpm.py:467), q_posterior
+    mean, noise scale exp(0.5 posterior_log_variance_clipped), no noise at t == 0, temperature 1.  One UNet replay and
+    one qd_ancestral_step per step."""
+
+    @torch.no_grad()
+    def sample(self, batch_size, shape, x_T=None, noise_fn=None, start_T=None, verbose=False, **kwargs):
+        sch = self.schedule
+        dev = torch.device("cuda", torch.cuda.current_device())
+        size = (batch_size,) + tuple(shape)
+        img = torch.randn(size, device=dev) if x_T is None else x_T.to(dev, torch.float32).clone()
+        nxt = torch.empty_like(img)
+        timesteps = sch.num_timesteps if start_T is None else min(sch.num_timesteps, start_T)
+        for k, i in enumerate(reversed(range(timesteps))):
+            ts = torch.full((batch_size,), i, device=dev, dtype=torch.long)
+            eps, _ = self._model_eps(img, ts, None, None, 1.)
+            noise = None
+            if i != 0:
+                noise = noise_fn(k, size, dev) if noise_fn is not None else torch.randn(size, device=dev)
+            _ancestral(img, eps, nxt, c_x=sch.sqrt_recip_alphas_cumprod[i], c_e=sch.sqrt_recipm1_alphas_cumprod[i],
+                       m_x0=sch.posterior_mean_coef1[i], m_x=sch.posterior_mean_coef2[i],
+                       sigma=torch.exp(0.5 * sch.posterior_log_variance_clipped[i]), noise=noise)
+            img, nxt = nxt, img
+        return img, {}
+
+
+# ------------------------------------------------------------------------------- singlestep DPM-Solver++
+def _interp(x, xp, yp):
+    """interpolate_fn (ddim/dpm_solver_pytorch.py:1261-1300) for increasing key points xp: piecewise linear, the outermost
+    segments extended beyond the ends."""
+    K = xp.shape[0]
+    xf = x.reshape(-1).contiguous()
+    idx = torch.searchsorted(xp, xf).clamp(1, K - 1)
+    x0, x1, y0, y1 = xp[idx - 1], xp[idx], yp[idx - 1], yp[idx]
+    return (y0 + (xf - x0) * (y1 - y0) / (x1 - x0)).reshape(x.shape)
+
+
+class _VPFromBetas:
+    """NoiseScheduleVP('discrete', betas=...) of the CIFAR script (ddim/dpm_solver_pytorch.py:100-170), fp32:
+    log_alpha = 0.5 cumsum(log(1 - beta)) on t_n = n / N -- not the LDM sampler's 0.5 log(alphas_cumprod)."""
+
+    def __init__(self, betas):
+        b = torch.as_tensor(betas).detach().cpu().to(torch.float32)
+        self.log_alpha = 0.5 * torch.log(1 - b).cumsum(dim=0)
+        self.total_N = b.shape[0]
+        self.t_array = torch.linspace(0., 1., self.total_N + 1)[1:]
+
+    def lm(self, t):
+        return _interp(t, self.t_array, self.log_alpha)
+
+    def alpha(self, t):
+        return torch.exp(self.lm(t))
+
+    def std(self, t):
+        return torch.sqrt(1. - torch.exp(2. * self.lm(t)))
+
+    def lam(self, t):
+        lm = self.lm(t)
+        return lm - 0.5 * torch.log(1. - torch.exp(2. * lm))
+
+    def inverse_lambda(self, lamb):
+        log_alpha = -0.5 * torch.logaddexp(torch.zeros((1,)), -2. * lamb)
+        return _interp(log_alpha, torch.flip(self.log_alpha, [0]), torch.flip(self.t_array, [0]))
+
+
+def singlestep_orders(steps, order=3):
+    """get_orders_and_timesteps_for_singlestep_solver (ddim/dpm_solver_pytorch.py:490-547): orders summing to `steps`."""
+    if order == 3:
+        K = steps // 3 + 1
+        return [3] * (K - 2) + [2, 1] if steps % 3 == 0 else [3] * (K - 1) + ([1] if steps % 3 == 1 else [2])
+    if order == 2:
+        return [2] * (steps // 2) + ([1] if steps % 2 else [])
+    if order == 1:
+        return [1] * steps
+    raise ValueError("'order' must be '1' or '2' or '3'.")
+
+
+@torch.no_grad()
+def dpm_solver_singlestep(x, model, betas, steps, order=3):
+    """`--sample_type dpm_solver` of the CIFAR script (scripts/sample_diffusion_ddim.py:310-325): DPM_Solver(...,
+    algorithm_type="dpmsolver++").sample(steps, order=3, skip_type="time_uniform", method="singlestep") of
+    ddim/dpm_solver_pytorch.py -- outer times linspace(1, 1/N, steps+1) at cumsum([0]+orders), r1 / r2 from each outer
+    step's inner time grid (:1229-1236), first / second / third singlestep updates in the 'dpmsolver' form (:555-760).
+    model(x, t) -> eps takes the fractional model time (t - 1/N) * 1000 (:279-291).  Each data prediction is the fused
+    qd_sampler_step x0 = (x - sigma_t eps) / alpha_t; each update is one qd_lincomb3 of at most three tensors.
+    NFE == steps.  Returns the final x."""
+    ns = _VPFromBetas(betas)
+    n, dev = x.size(0), x.device
+    orders = singlestep_orders(steps, order)
+    t_0, t_T = 1. / ns.total_N, 1.
+    outer = torch.linspace(t_T, t_0, steps + 1)[torch.cumsum(torch.tensor([0] + orders), 0)]
+    cur = x.to(torch.float32).clone()
+    nxt, xi, scratch = torch.empty_like(cur), torch.empty_like(cur), torch.empty_like(cur)
+    ms = [torch.empty_like(cur) for _ in range(3)]
+
+    def data_pred(xx, t, out):
+        a, sg = ns.alpha(t), ns.std(t)
+        t_in = torch.full((n,), float((t.reshape(-1)[0] - 1. / ns.total_N) * 1000.), device=dev, dtype=torch.float32)
+        eps = model(xx, t_in)
+        _step(xx, eps, scratch, a_t=float(a) ** 2, a_prev=1.0, sigma=0.0, sqrt_one_minus_at=float(sg), pred_x0=out)
+        return out
+
+    for step, o in enumerate(orders):
+        s, t = outer[step], outer[step + 1]
+        lam_in = ns.lam(torch.linspace(s.item(), t.item(), o + 1))
+        h_in = lam_in[-1] - lam_in[0]
+        l_s, l_t = ns.lam(s), ns.lam(t)
+        h = l_t - l_s
+        sg_s, sg_t, a_t = ns.std(s), ns.std(t), ns.alpha(t)
+        phi_1 = torch.expm1(-h)
+        m_s = data_pred(cur, s, ms[0])
+        if o == 1:
+            ops.lincomb3(nxt, float(sg_t / sg_s), cur, float(-(a_t * phi_1)), m_s)
+        else:
+            r1 = (lam_in[1] - lam_in[0]) / h_in
+            s1 = ns.inverse_lambda(l_s + r1 * h)
+            a_s1, sg_s1 = ns.alpha(s1), ns.std(s1)
+            ops.lincomb3(xi, float(sg_s1 / sg_s), cur, float(-(a_s1 * torch.expm1(-r1 * h))), m_s)
+            m_s1 = data_pred(xi, s1, ms[1])
+            if o == 2:
+                # x_t = (sg_t/sg_s) x - k m_s - (0.5/r1) k (m_s1 - m_s),  k = alpha_t phi_1
+                k = a_t * phi_1
+                ops.lincomb3(nxt, float(sg_t / sg_s), cur, float(-k + (0.5 / r1) * k), m_s, float(-(0.5 / r1) * k), m_s1)
+            else:
+                r2 = (lam_in[2] - lam_in[0]) / h_in
+                s2 = ns.inverse_lambda(l_s + r2 * h)
+                a_s2, sg_s2 = ns.alpha(s2), ns.std(s2)
+                phi_12 = torch.expm1(-r2 * h)
+                phi_22 = torch.expm1(-r2 * h) / (r2 * h) + 1.
+                phi_2 = phi_1 / h + 1.
+                # x_s2 = (sg_s2/sg_s) x - a_s2 phi_12 m_s + c (m_s1 - m_s),  c = r2/r1 a_s2 phi_22
+                c = r2 / r1 * (a_s2 * phi_22)
+                ops.lincomb3(xi, float(sg_s2 / sg_s), cur, float(-(a_s2 * phi_12) - c), m_s, float(c), m_s1)
+                m_s2 = data_pred(xi, s2, ms[2])
+                # x_t = (sg_t/sg_s) x - a_t phi_1 m_s + k2 (m_s2 - m_s),  k2 = a_t phi_2 / r2
+                k2 = (1. / r2) * (a_t * phi_2)
+                ops.lincomb3(nxt, float(sg_t / sg_s), cur, float(-(a_t * phi_1) - k2), m_s, float(k2), m_s2)
         cur, nxt = nxt, cur
     return cur
