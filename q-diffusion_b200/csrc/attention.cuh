@@ -21,6 +21,7 @@
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
+#include <type_traits>
 #include "../../include/qdiff_b200.h"
 #include "quant_math.cuh"
 
@@ -132,6 +133,20 @@ __device__ __forceinline__ float att_i2f(int s) {
   else return (float)s;
 }
 
+// Score type of the two-pass kernels: int32 on 8-bit codes; on fp16 operands the fp32 accumulators, which already hold
+// the exact integer scores (|S| < 2^22), so they skip the float -> int -> float round trip (F2I on the XU pipe).  Every
+// value, maximum and exponent argument is the same in both forms.
+template <bool F16>
+using att_score_t = std::conditional_t<F16, float, int>;
+template <bool MAGIC>
+__device__ __forceinline__ float att_s2f(int s) { return att_i2f<MAGIC>(s); }
+template <bool MAGIC>
+__device__ __forceinline__ float att_s2f(float s) { return s; }
+__device__ __forceinline__ int att_smax(int a, int b) { return max(a, b); }
+__device__ __forceinline__ float att_smax(float a, float b) { return fmaxf(a, b); }
+__device__ __forceinline__ int att_lowest(int) { return INT_MIN; }
+__device__ __forceinline__ float att_lowest(float) { return -INFINITY; }
+
 // DQ: reduction length of QK^T padded to a multiple of 32; DV: head dim d (multiple of 8).
 // Shared-memory tiles are addressed from the array symbol (the
 // pointer-array version compiled to generic LD + 64-bit IMAD address math), the
@@ -220,7 +235,8 @@ qattention_kernel(const qd_attention_desc p) {
   const bool has_zq = !F16 && p.zq != 0;
   const bool ragged = (p.Tk % ATT_BN) != 0;
 
-  int mi0 = INT_MIN, mi1 = INT_MIN;   // running integer row maxima (of S_raw - zrk)
+  using SV = att_score_t<F16>;
+  SV mi0 = att_lowest(SV{}), mi1 = att_lowest(SV{});   // running integer row maxima (of S_raw - zrk)
   float l0 = 0.f, l1 = 0.f;           // running sums of exp2((S - max) * c)
   float off0 = 0.f, off1 = 0.f;       // pass-2 exponent offsets
   int olo[NDT][4], ohi[SM16 ? NDT : 1][4];
@@ -252,22 +268,17 @@ qattention_kernel(const qd_attention_desc p) {
       const uint8_t* sV = att_smem + 2 * KB + buf * VB;
       const int* sZrk = reinterpret_cast<const int*>(att_smem + 2 * KB + 2 * VB + buf * ZB);
 
-      // ---- S = Q K^T for this warp: 16 x 64 (int32)
-      int sacc[8][4];
+      // ---- S = Q K^T for this warp: 16 x 64 (int32, or exact integers in fp32 on fp16 operands)
+      SV sacc[8][4];
 #pragma unroll
       for (int nt = 0; nt < 8; ++nt) {
         sacc[nt][0] = sacc[nt][1] = sacc[nt][2] = sacc[nt][3] = 0;
-        [[maybe_unused]] float facc[4] = {0.f, 0.f, 0.f, 0.f};
 #pragma unroll
         for (int kc = 0; kc < NKC; ++kc) {
           const uint2 kk = *reinterpret_cast<const uint2*>(sK + (8 * nt + g) * KP + kc * 32 + 8 * t);
           const uint32_t bf[2] = {kk.x, kk.y};
-          if constexpr (F16) mma_f16_16816(facc, qf[kc], bf);
+          if constexpr (F16) mma_f16_16816(sacc[nt], qf[kc], bf);
           else mma_i8_16832<QK_SIGNED, QK_SIGNED>(sacc[nt], qf[kc], bf);
-        }
-        if constexpr (F16) {     // exact integers in fp32
-          sacc[nt][0] = __float2int_rn(facc[0]); sacc[nt][1] = __float2int_rn(facc[1]);
-          sacc[nt][2] = __float2int_rn(facc[2]); sacc[nt][3] = __float2int_rn(facc[3]);
         }
       }
       if (has_zq) {
@@ -286,24 +297,24 @@ qattention_kernel(const qd_attention_desc p) {
         }
       }
       if (pass == 0) {
-        int tm0 = sacc[0][0], tm1 = sacc[0][2];
+        SV tm0 = sacc[0][0], tm1 = sacc[0][2];
 #pragma unroll
         for (int nt = 0; nt < 8; ++nt) {
-          tm0 = max(tm0, max(sacc[nt][0], sacc[nt][1]));
-          tm1 = max(tm1, max(sacc[nt][2], sacc[nt][3]));
+          tm0 = att_smax(tm0, att_smax(sacc[nt][0], sacc[nt][1]));
+          tm1 = att_smax(tm1, att_smax(sacc[nt][2], sacc[nt][3]));
         }
-        tm0 = max(tm0, __shfl_xor_sync(0xffffffffu, tm0, 1));
-        tm0 = max(tm0, __shfl_xor_sync(0xffffffffu, tm0, 2));
-        tm1 = max(tm1, __shfl_xor_sync(0xffffffffu, tm1, 1));
-        tm1 = max(tm1, __shfl_xor_sync(0xffffffffu, tm1, 2));
-        if (tm0 > mi0) { l0 *= (mi0 == INT_MIN) ? 0.f : ex2_approx((float)(mi0 - tm0) * c); mi0 = tm0; }
-        if (tm1 > mi1) { l1 *= (mi1 == INT_MIN) ? 0.f : ex2_approx((float)(mi1 - tm1) * c); mi1 = tm1; }
+        tm0 = att_smax(tm0, __shfl_xor_sync(0xffffffffu, tm0, 1));
+        tm0 = att_smax(tm0, __shfl_xor_sync(0xffffffffu, tm0, 2));
+        tm1 = att_smax(tm1, __shfl_xor_sync(0xffffffffu, tm1, 1));
+        tm1 = att_smax(tm1, __shfl_xor_sync(0xffffffffu, tm1, 2));
+        if (tm0 > mi0) { l0 *= (mi0 == att_lowest(SV{})) ? 0.f : ex2_approx((float)(mi0 - tm0) * c); mi0 = tm0; }
+        if (tm1 > mi1) { l1 *= (mi1 == att_lowest(SV{})) ? 0.f : ex2_approx((float)(mi1 - tm1) * c); mi1 = tm1; }
         const float b0 = -(float)mi0 * c, b1 = -(float)mi1 * c;
         float a0 = 0.f, a1 = 0.f;
 #pragma unroll
         for (int nt = 0; nt < 8; ++nt) {
-          a0 += ex2_approx(fmaf(att_i2f<MAGIC>(sacc[nt][0]), c, b0)) + ex2_approx(fmaf(att_i2f<MAGIC>(sacc[nt][1]), c, b0));
-          a1 += ex2_approx(fmaf(att_i2f<MAGIC>(sacc[nt][2]), c, b1)) + ex2_approx(fmaf(att_i2f<MAGIC>(sacc[nt][3]), c, b1));
+          a0 += ex2_approx(fmaf(att_s2f<MAGIC>(sacc[nt][0]), c, b0)) + ex2_approx(fmaf(att_s2f<MAGIC>(sacc[nt][1]), c, b0));
+          a1 += ex2_approx(fmaf(att_s2f<MAGIC>(sacc[nt][2]), c, b1)) + ex2_approx(fmaf(att_s2f<MAGIC>(sacc[nt][3]), c, b1));
         }
         l0 += a0;
         l1 += a1;
@@ -317,11 +328,11 @@ qattention_kernel(const qd_attention_desc p) {
           for (int half = 0; half < 2; ++half) {      // a0/a1 (keys 0..15 of the chunk) then a2/a3 (16..31)
             const int ntA = 4 * kc + 2 * half, ntB = ntA + 1;
             uint32_t cd[8];
-            const int sv[8] = {sacc[ntA][0], sacc[ntA][1], sacc[ntB][0], sacc[ntB][1],
-                               sacc[ntA][2], sacc[ntA][3], sacc[ntB][2], sacc[ntB][3]};
+            const SV sv[8] = {sacc[ntA][0], sacc[ntA][1], sacc[ntB][0], sacc[ntB][1],
+                              sacc[ntA][2], sacc[ntA][3], sacc[ntB][2], sacc[ntB][3]};
 #pragma unroll
             for (int e = 0; e < 8; ++e) {
-              const float pr = ex2_approx(fmaf(att_i2f<MAGIC>(sv[e]), c, e < 4 ? off0 : off1));
+              const float pr = ex2_approx(fmaf(att_s2f<MAGIC>(sv[e]), c, e < 4 ? off0 : off1));
               cd[e] = __float_as_uint(fminf(pr, pmax) + 12582912.0f);
             }
             plo[2 * half] = __byte_perm(__byte_perm(cd[0], cd[1], 0x0040), __byte_perm(cd[2], cd[3], 0x0040), 0x5410);

@@ -5,8 +5,10 @@
 //   * O += P V as wgmma m64nNV k32 (u8 P codes in registers, V^T tile in shared memory), NV = d + 8 rounded up to a
 //     wgmma width (the extra rows: the all-ones row, then zeros);
 //   * K, V^T and the zq*rowsum(k) slice staged by TMA / bulk copies through an ATW_STAGES-deep mbarrier ring (one load
-//     per (pass, key tile); pass 0 needs no V^T).
-// Two consumer warpgroups, 64 query rows each.  The per-warp accumulator fragment of wgmma m64nN is the m16n8 fragment
+//     per (pass, key tile); pass 0 needs no V^T).  The consumer warp that releases a stage last refills it.
+// Two consumer warpgroups, 64 query rows each, running the loads L = 0 .. 2*ntiles-1 of both passes in one sequence;
+// for d <= 40 two CTAs share an SM (MINB = 2, <= 128 registers).  On fp16 operands the fp32 scores are used as they are
+// (exact integers), with no conversion to int32.  The per-warp accumulator fragment of wgmma m64nN is the m16n8 fragment
 // of mma.sync repeated over N / 8 column tiles, and the register A operand has the m16n8k32 layout, so the softmax code
 // below is qattention_kernel's, operating on the same registers.  V^T keeps its 16-key byte permutation
 // (att_vt_perm): with it, the P fragments built from the S accumulators are the A operand without shuffles.
@@ -161,7 +163,7 @@ __device__ __forceinline__ void wgmma_ra_u8s8_n112(uint32_t* d, const uint32_t (
       : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(scale_d));
 }
 
-constexpr int ATW_STAGES = 3;
+constexpr int ATW_STAGES = 4;
 constexpr int ATW_THREADS = ATT_WARPS * 32;       // two warpgroups
 // PV width: d + 8 (the all-ones row sits at row d) rounded up to a wgmma N for 8-bit operands
 __host__ __device__ constexpr int atw_nv(int DV) {
@@ -177,7 +179,7 @@ __host__ __device__ inline AtwSmem atw_smem(int P, int NV) {
   l.v_bytes = (NV * ATT_BN + 1023) / 1024 * 1024;
   l.z_off = ATW_STAGES * (l.k_bytes + l.v_bytes);
   l.bar_off = l.z_off + ATW_STAGES * ATT_BN * 4;
-  l.total = l.bar_off + 2 * ATW_STAGES * 8 + 1024;   // + alignment slack
+  l.total = l.bar_off + ATW_STAGES * 8 + ATW_STAGES * 4 + 1024;   // full barriers, release counters, alignment slack
   return l;
 }
 // sm_90 shared-memory descriptor for a K-major tile of `row_bytes`-byte rows stored with the matching TMA swizzle
@@ -191,30 +193,30 @@ __device__ __forceinline__ uint64_t atw_desc(uint32_t addr, int row_bytes) {
 }
 
 template <int N, bool VS>
-__device__ __forceinline__ void atw_pv(uint32_t* d, const uint32_t (&a)[4], uint64_t db) {
+__device__ __forceinline__ void atw_pv(uint32_t* d, const uint32_t (&a)[4], uint64_t db, uint32_t scale_d) {
   if constexpr (VS) {
-    if constexpr (N == 24) wgmma_ra_u8s8_n24(d, a, db, 1u);
-    else if constexpr (N == 32) wgmma_ra_u8s8_n32(d, a, db, 1u);
-    else if constexpr (N == 48) wgmma_ra_u8s8_n48(d, a, db, 1u);
-    else if constexpr (N == 64) wgmma_ra_u8s8_n64(d, a, db, 1u);
-    else if constexpr (N == 80) wgmma_ra_u8s8_n80(d, a, db, 1u);
-    else if constexpr (N == 96) wgmma_ra_u8s8_n96(d, a, db, 1u);
-    else wgmma_ra_u8s8_n112(d, a, db, 1u);
+    if constexpr (N == 24) wgmma_ra_u8s8_n24(d, a, db, scale_d);
+    else if constexpr (N == 32) wgmma_ra_u8s8_n32(d, a, db, scale_d);
+    else if constexpr (N == 48) wgmma_ra_u8s8_n48(d, a, db, scale_d);
+    else if constexpr (N == 64) wgmma_ra_u8s8_n64(d, a, db, scale_d);
+    else if constexpr (N == 80) wgmma_ra_u8s8_n80(d, a, db, scale_d);
+    else if constexpr (N == 96) wgmma_ra_u8s8_n96(d, a, db, scale_d);
+    else wgmma_ra_u8s8_n112(d, a, db, scale_d);
   } else {
-    if constexpr (N == 24) wgmma_ra_u8u8_n24(d, a, db, 1u);
-    else if constexpr (N == 32) wgmma_ra_u8u8_n32(d, a, db, 1u);
-    else if constexpr (N == 48) wgmma_ra_u8u8_n48(d, a, db, 1u);
-    else if constexpr (N == 64) wgmma_ra_u8u8_n64(d, a, db, 1u);
-    else if constexpr (N == 80) wgmma_ra_u8u8_n80(d, a, db, 1u);
-    else if constexpr (N == 96) wgmma_ra_u8u8_n96(d, a, db, 1u);
-    else wgmma_ra_u8u8_n112(d, a, db, 1u);
+    if constexpr (N == 24) wgmma_ra_u8u8_n24(d, a, db, scale_d);
+    else if constexpr (N == 32) wgmma_ra_u8u8_n32(d, a, db, scale_d);
+    else if constexpr (N == 48) wgmma_ra_u8u8_n48(d, a, db, scale_d);
+    else if constexpr (N == 64) wgmma_ra_u8u8_n64(d, a, db, scale_d);
+    else if constexpr (N == 80) wgmma_ra_u8u8_n80(d, a, db, scale_d);
+    else if constexpr (N == 96) wgmma_ra_u8u8_n96(d, a, db, scale_d);
+    else wgmma_ra_u8u8_n112(d, a, db, scale_d);
   }
 }
 
 // DQ: bytes of the padded QK^T reduction (multiple of 32, <= P); DV: head dim d; P: per-head pitch of Q / K in bytes
 // (32 / 64 / 128, also the K tile's swizzle span).
-template <int DQ, int DV, bool QK_SIGNED, bool V_SIGNED, bool SM16, bool F16>
-__global__ void __launch_bounds__(ATW_THREADS, 1)
+template <int DQ, int DV, bool QK_SIGNED, bool V_SIGNED, bool SM16, bool F16, int MINB>
+__global__ void __launch_bounds__(ATW_THREADS, MINB)
 qattention_wg_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_constant__ CUtensorMap tmV,
                      const qd_attention_desc p, int P) {
   constexpr int NV = atw_nv(DV);
@@ -223,11 +225,12 @@ qattention_wg_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_const
   constexpr bool MAGIC = DV <= 64;  // |S| <= 255*255*d < 2^22
   constexpr int RB = F16 ? 2 * DV : DV;   // bytes of one head's Q / K row
   static_assert(!F16 || DV <= 64, "fp16 Q / K operands: d <= 64 keeps |S| below 2^22");
+  using SV = att_score_t<F16>;      // score: int32, or the exact fp32 accumulator
   extern __shared__ uint8_t atw_raw[];
   uint8_t* smem = atw_raw + (((smem_u32(atw_raw) + 1023u) & ~1023u) - smem_u32(atw_raw));
   const AtwSmem lay = atw_smem(P, NV);
   uint64_t* full = reinterpret_cast<uint64_t*>(smem + lay.bar_off);
-  uint64_t* empty = full + ATW_STAGES;
+  int* released = reinterpret_cast<int*>(full + ATW_STAGES);   // per stage: consumer-warp releases so far
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int g = lane >> 2, t = lane & 3;
@@ -250,14 +253,14 @@ qattention_wg_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_const
     tma_prefetch_desc(&tmV);
     for (int s = 0; s < ATW_STAGES; ++s) {
       mbar_init(&full[s], 1);
-      mbar_init(&empty[s], ATT_WARPS);
+      released[s] = 0;
     }
     fence_mbar_init();
   }
   fence_proxy_async();     // the generic writes above -> visible to the tensor cores
   __syncthreads();
 
-  auto issue = [&](int L) {           // thread 0: load number L into stage L % ATW_STAGES
+  auto issue = [&](int L) {           // one thread: load number L into stage L % ATW_STAGES
     const int s = L % ATW_STAGES, pass = L / ntiles, tile = L - pass * ntiles;
     const int j0 = tile * ATT_BN;
     const uint32_t bytes = (uint32_t)(ATT_BN * P) + (pass ? (uint32_t)(ATT_BN * DV) : 0u) + (has_zq ? ATT_BN * 4u : 0u);
@@ -288,19 +291,48 @@ qattention_wg_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_const
   }
   const float c = p.sim_scale * 1.4426950408889634f;
   const bool ragged = (p.Tk % ATT_BN) != 0;
-  int mi0 = INT_MIN, mi1 = INT_MIN;
+  SV mi0 = att_lowest(SV{}), mi1 = att_lowest(SV{});
   float l0 = 0.f, l1 = 0.f;
   float off0 = 0.f, off1 = 0.f;
-  uint32_t olo[NV / 2], ohi[SM16 ? NV / 2 : 1];
-#pragma unroll
-  for (int i = 0; i < NV / 2; ++i) olo[i] = 0u;
-#pragma unroll
-  for (int i = 0; i < (SM16 ? NV / 2 : 1); ++i) ohi[i] = 0u;
+  uint32_t olo[NV / 2], ohi[SM16 ? NV / 2 : 1];     // zeroed by the first PV (scale_d = 0)
   const float pmax = (float)p.p_qmax;
   const QuantK oqk = make_quantk(p.oq);
 
-  for (int pass = 0; pass < 2; ++pass) {
-    if (pass == 1) {
+  // S(L) = Q K^T for this warpgroup, 64 x 64, once load L has landed; this warp's 16 rows land in s[nt][0..3]
+  // (m16n8 fragments)
+  auto issue_s = [&](SV (&s)[8][4], int L) {
+    const int st = L % ATW_STAGES;
+    mbar_wait(&full[st], (uint32_t)(L / ATW_STAGES) & 1u);
+    const uint64_t dK = atw_desc(smem_u32(smem + st * lay.k_bytes), P);
+    wgmma_fence();
+#pragma unroll
+    for (int kc = 0; kc < NKC; ++kc) {
+      if constexpr (F16) wgmma_ra_f16_n64(&s[0][0], qf[kc], dK + (uint64_t)(2 * kc), kc ? 1u : 0u);
+      else if constexpr (QK_SIGNED) wgmma_ra_s8s8_n64(reinterpret_cast<uint32_t*>(&s[0][0]), qf[kc], dK + (uint64_t)(2 * kc), kc ? 1u : 0u);
+      else wgmma_ra_u8u8_n64(reinterpret_cast<uint32_t*>(&s[0][0]), qf[kc], dK + (uint64_t)(2 * kc), kc ? 1u : 0u);
+    }
+    wgmma_commit();
+  };
+
+  // Release load R; the last of the 8 warps to do so refills the stage, so no warp waits for another.
+  auto release = [&](int R) {
+    __syncwarp();
+    if (lane == 0) {
+      const int s = R % ATW_STAGES;
+      __threadfence_block();
+      const int n = atomicAdd(&released[s], 1);
+      if (n == ATT_WARPS * (R / ATW_STAGES + 1) - 1 && R + ATW_STAGES < nloads) {
+        __threadfence_block();
+        issue(R + ATW_STAGES);
+      }
+    }
+  };
+
+  // Softmax of the completed scores S(L) (edited in place) and, in pass 1, PV(L) issued and committed.
+  auto softmax_pv = [&](SV (&sacc)[8][4], int L) {
+    const int pass = L >= ntiles ? 1 : 0, tile = L - pass * ntiles, st = L % ATW_STAGES;
+    const int j0 = tile * ATT_BN;
+    if (L == ntiles) {
       l0 += __shfl_xor_sync(0xffffffffu, l0, 1);
       l0 += __shfl_xor_sync(0xffffffffu, l0, 2);
       l1 += __shfl_xor_sync(0xffffffffu, l1, 1);
@@ -308,125 +340,100 @@ qattention_wg_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_const
       off0 = -(float)mi0 * c + log2f(1.0f / (l0 * p.delta_w));
       off1 = -(float)mi1 * c + log2f(1.0f / (l1 * p.delta_w));
     }
-    for (int tile = 0; tile < ntiles; ++tile) {
-      const int L = pass * ntiles + tile, st = L % ATW_STAGES;
-      const uint32_t ph = (uint32_t)(L / ATW_STAGES) & 1u;
-      const int j0 = tile * ATT_BN;
-      mbar_wait(&full[st], ph);
-      const uint64_t dK = atw_desc(smem_u32(smem + st * lay.k_bytes), P);
-      const int* sZrk = reinterpret_cast<const int*>(smem + lay.z_off + st * ATT_BN * 4);
-
-      // ---- S = Q K^T for this warpgroup: 64 x 64; this warp's 16 rows land in sacc[nt][*] (m16n8 fragments)
-      int sacc[8][4];
-      {
-        uint32_t si[32];
-        float sf[F16 ? 32 : 1];
-        wgmma_fence();
+    const int* sZrk = reinterpret_cast<const int*>(smem + lay.z_off + st * ATT_BN * 4);
+    if (has_zq) {
 #pragma unroll
-        for (int kc = 0; kc < NKC; ++kc) {
-          if constexpr (F16) wgmma_ra_f16_n64(sf, qf[kc], dK + (uint64_t)(2 * kc), kc ? 1u : 0u);
-          else if constexpr (QK_SIGNED) wgmma_ra_s8s8_n64(si, qf[kc], dK + (uint64_t)(2 * kc), kc ? 1u : 0u);
-          else wgmma_ra_u8u8_n64(si, qf[kc], dK + (uint64_t)(2 * kc), kc ? 1u : 0u);
-        }
-        wgmma_commit();
-        wgmma_wait<0>();
-        if constexpr (F16) {
-#pragma unroll
-          for (int i = 0; i < 32; ++i) asm volatile("" : "+f"(sf[i])::"memory");
-#pragma unroll
-          for (int i = 0; i < 32; ++i) sacc[i >> 2][i & 3] = __float2int_rn(sf[i]);     // exact integers
-        } else {
-#pragma unroll
-          for (int i = 0; i < 32; ++i) asm volatile("" : "+r"(si[i])::"memory");
-#pragma unroll
-          for (int i = 0; i < 32; ++i) sacc[i >> 2][i & 3] = (int)si[i];
-        }
+      for (int nt = 0; nt < 8; ++nt) {
+        const int2 z = *reinterpret_cast<const int2*>(sZrk + 8 * nt + 2 * t);
+        sacc[nt][0] -= z.x; sacc[nt][1] -= z.y; sacc[nt][2] -= z.x; sacc[nt][3] -= z.y;
       }
-      if (has_zq) {
+    }
+    if (ragged && tile == ntiles - 1) {
 #pragma unroll
-        for (int nt = 0; nt < 8; ++nt) {
-          const int2 z = *reinterpret_cast<const int2*>(sZrk + 8 * nt + 2 * t);
-          sacc[nt][0] -= z.x; sacc[nt][1] -= z.y; sacc[nt][2] -= z.x; sacc[nt][3] -= z.y;
-        }
+      for (int nt = 0; nt < 8; ++nt) {
+        const int j = j0 + 8 * nt + 2 * t;
+        if (j >= p.Tk) { sacc[nt][0] = -(1 << 21); sacc[nt][2] = -(1 << 21); }
+        if (j + 1 >= p.Tk) { sacc[nt][1] = -(1 << 21); sacc[nt][3] = -(1 << 21); }
       }
-      if (ragged && tile == ntiles - 1) {
+    }
+    if (pass == 0) {
+      SV tm0 = sacc[0][0], tm1 = sacc[0][2];
 #pragma unroll
-        for (int nt = 0; nt < 8; ++nt) {
-          const int j = j0 + 8 * nt + 2 * t;
-          if (j >= p.Tk) { sacc[nt][0] = -(1 << 21); sacc[nt][2] = -(1 << 21); }
-          if (j + 1 >= p.Tk) { sacc[nt][1] = -(1 << 21); sacc[nt][3] = -(1 << 21); }
-        }
+      for (int nt = 0; nt < 8; ++nt) {
+        tm0 = att_smax(tm0, att_smax(sacc[nt][0], sacc[nt][1]));
+        tm1 = att_smax(tm1, att_smax(sacc[nt][2], sacc[nt][3]));
       }
-      if (pass == 0) {
-        int tm0 = sacc[0][0], tm1 = sacc[0][2];
+      tm0 = att_smax(tm0, __shfl_xor_sync(0xffffffffu, tm0, 1));
+      tm0 = att_smax(tm0, __shfl_xor_sync(0xffffffffu, tm0, 2));
+      tm1 = att_smax(tm1, __shfl_xor_sync(0xffffffffu, tm1, 1));
+      tm1 = att_smax(tm1, __shfl_xor_sync(0xffffffffu, tm1, 2));
+      if (tm0 > mi0) { l0 *= (mi0 == att_lowest(SV{})) ? 0.f : ex2_approx((float)(mi0 - tm0) * c); mi0 = tm0; }
+      if (tm1 > mi1) { l1 *= (mi1 == att_lowest(SV{})) ? 0.f : ex2_approx((float)(mi1 - tm1) * c); mi1 = tm1; }
+      const float b0 = -(float)mi0 * c, b1 = -(float)mi1 * c;
+      float a0 = 0.f, a1 = 0.f;
 #pragma unroll
-        for (int nt = 0; nt < 8; ++nt) {
-          tm0 = max(tm0, max(sacc[nt][0], sacc[nt][1]));
-          tm1 = max(tm1, max(sacc[nt][2], sacc[nt][3]));
-        }
-        tm0 = max(tm0, __shfl_xor_sync(0xffffffffu, tm0, 1));
-        tm0 = max(tm0, __shfl_xor_sync(0xffffffffu, tm0, 2));
-        tm1 = max(tm1, __shfl_xor_sync(0xffffffffu, tm1, 1));
-        tm1 = max(tm1, __shfl_xor_sync(0xffffffffu, tm1, 2));
-        if (tm0 > mi0) { l0 *= (mi0 == INT_MIN) ? 0.f : ex2_approx((float)(mi0 - tm0) * c); mi0 = tm0; }
-        if (tm1 > mi1) { l1 *= (mi1 == INT_MIN) ? 0.f : ex2_approx((float)(mi1 - tm1) * c); mi1 = tm1; }
-        const float b0 = -(float)mi0 * c, b1 = -(float)mi1 * c;
-        float a0 = 0.f, a1 = 0.f;
+      for (int nt = 0; nt < 8; ++nt) {
+        a0 += ex2_approx(fmaf(att_s2f<MAGIC>(sacc[nt][0]), c, b0)) + ex2_approx(fmaf(att_s2f<MAGIC>(sacc[nt][1]), c, b0));
+        a1 += ex2_approx(fmaf(att_s2f<MAGIC>(sacc[nt][2]), c, b1)) + ex2_approx(fmaf(att_s2f<MAGIC>(sacc[nt][3]), c, b1));
+      }
+      l0 += a0;
+      l1 += a1;
+    } else {
+      // ---- P codes packed straight into A fragments (byte planes), then O += P V on the warpgroup, left in flight
+      const uint64_t dV = atw_desc(smem_u32(smem + ATW_STAGES * lay.k_bytes + st * lay.v_bytes), ATT_BN);
+      uint32_t plo[2][4], phi[2][4];
 #pragma unroll
-        for (int nt = 0; nt < 8; ++nt) {
-          a0 += ex2_approx(fmaf(att_i2f<MAGIC>(sacc[nt][0]), c, b0)) + ex2_approx(fmaf(att_i2f<MAGIC>(sacc[nt][1]), c, b0));
-          a1 += ex2_approx(fmaf(att_i2f<MAGIC>(sacc[nt][2]), c, b1)) + ex2_approx(fmaf(att_i2f<MAGIC>(sacc[nt][3]), c, b1));
-        }
-        l0 += a0;
-        l1 += a1;
-      } else {
-        // ---- P codes packed straight into A fragments (byte planes), then O += P V on the warpgroup
-        const uint64_t dV = atw_desc(smem_u32(smem + ATW_STAGES * lay.k_bytes + st * lay.v_bytes), ATT_BN);
-        uint32_t plo[2][4], phi[2][4];
+      for (int kc = 0; kc < 2; ++kc) {
 #pragma unroll
-        for (int kc = 0; kc < 2; ++kc) {
+        for (int half = 0; half < 2; ++half) {
+          const int ntA = 4 * kc + 2 * half, ntB = ntA + 1;
+          uint32_t cd[8];
+          const SV sv[8] = {sacc[ntA][0], sacc[ntA][1], sacc[ntB][0], sacc[ntB][1],
+                            sacc[ntA][2], sacc[ntA][3], sacc[ntB][2], sacc[ntB][3]};
 #pragma unroll
-          for (int half = 0; half < 2; ++half) {
-            const int ntA = 4 * kc + 2 * half, ntB = ntA + 1;
-            uint32_t cd[8];
-            const int sv[8] = {sacc[ntA][0], sacc[ntA][1], sacc[ntB][0], sacc[ntB][1],
-                               sacc[ntA][2], sacc[ntA][3], sacc[ntB][2], sacc[ntB][3]};
-#pragma unroll
-            for (int e = 0; e < 8; ++e) {
-              const float pr = ex2_approx(fmaf(att_i2f<MAGIC>(sv[e]), c, e < 4 ? off0 : off1));
-              cd[e] = __float_as_uint(fminf(pr, pmax) + 12582912.0f);
-            }
-            plo[kc][2 * half] = __byte_perm(__byte_perm(cd[0], cd[1], 0x0040), __byte_perm(cd[2], cd[3], 0x0040), 0x5410);
-            plo[kc][2 * half + 1] = __byte_perm(__byte_perm(cd[4], cd[5], 0x0040), __byte_perm(cd[6], cd[7], 0x0040), 0x5410);
-            if constexpr (SM16) {
-              phi[kc][2 * half] = __byte_perm(__byte_perm(cd[0], cd[1], 0x0051), __byte_perm(cd[2], cd[3], 0x0051), 0x5410);
-              phi[kc][2 * half + 1] = __byte_perm(__byte_perm(cd[4], cd[5], 0x0051), __byte_perm(cd[6], cd[7], 0x0051), 0x5410);
-            }
+          for (int e = 0; e < 8; ++e) {
+            const float pr = ex2_approx(fmaf(att_s2f<MAGIC>(sv[e]), c, e < 4 ? off0 : off1));
+            cd[e] = __float_as_uint(fminf(pr, pmax) + 12582912.0f);
+          }
+          plo[kc][2 * half] = __byte_perm(__byte_perm(cd[0], cd[1], 0x0040), __byte_perm(cd[2], cd[3], 0x0040), 0x5410);
+          plo[kc][2 * half + 1] = __byte_perm(__byte_perm(cd[4], cd[5], 0x0040), __byte_perm(cd[6], cd[7], 0x0040), 0x5410);
+          if constexpr (SM16) {
+            phi[kc][2 * half] = __byte_perm(__byte_perm(cd[0], cd[1], 0x0051), __byte_perm(cd[2], cd[3], 0x0051), 0x5410);
+            phi[kc][2 * half + 1] = __byte_perm(__byte_perm(cd[4], cd[5], 0x0051), __byte_perm(cd[6], cd[7], 0x0051), 0x5410);
           }
         }
-        wgmma_fence();
-#pragma unroll
-        for (int kc = 0; kc < 2; ++kc) {
-          atw_pv<NV, V_SIGNED>(olo, plo[kc], dV + (uint64_t)(2 * kc));
-          if constexpr (SM16) atw_pv<NV, V_SIGNED>(ohi, phi[kc], dV + (uint64_t)(2 * kc));
-        }
-        wgmma_commit();
-        wgmma_wait<0>();
-#pragma unroll
-        for (int i = 0; i < NV / 2; ++i) asm volatile("" : "+r"(olo[i])::"memory");
-#pragma unroll
-        for (int i = 0; i < (SM16 ? NV / 2 : 1); ++i) asm volatile("" : "+r"(ohi[i])::"memory");
       }
-      // ---- this warp is done with the stage; thread 0 refills it once every warp is
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&empty[st]);
-      if (threadIdx.x == 0 && L + ATW_STAGES < nloads) {
-        mbar_wait(&empty[st], ph);
-        issue(L + ATW_STAGES);
+      wgmma_fence();
+#pragma unroll
+      for (int kc = 0; kc < 2; ++kc) {
+        const uint32_t acc = (kc || L > ntiles) ? 1u : 0u;
+        atw_pv<NV, V_SIGNED>(olo, plo[kc], dV + (uint64_t)(2 * kc), acc);
+        if constexpr (SM16) atw_pv<NV, V_SIGNED>(ohi, phi[kc], dV + (uint64_t)(2 * kc), acc);
       }
-      __syncwarp();
+      wgmma_commit();
     }
+  };
+
+  // One S register set, every wgmma retired before the next load: few enough registers that, for d <= 40, two CTAs
+  // share an SM and their warps hide each other's latencies (measured: faster than overlapping S(L+1) and PV(L) with
+  // the softmax inside one CTA, which needs a second S set; DESIGN §6).
+  for (int L = 0; L < nloads; ++L) {
+    SV sacc[8][4];
+    issue_s(sacc, L);
+    wgmma_wait<0>();
+#pragma unroll
+    for (int i = 0; i < 32; ++i) {
+      if constexpr (F16) asm volatile("" : "+f"(sacc[i >> 2][i & 3])::"memory");
+      else asm volatile("" : "+r"(sacc[i >> 2][i & 3])::"memory");
+    }
+    softmax_pv(sacc, L);
+    wgmma_wait<0>();
+    release(L);
   }
+#pragma unroll
+  for (int i = 0; i < NV / 2; ++i) asm volatile("" : "+r"(olo[i])::"memory");
+#pragma unroll
+  for (int i = 0; i < (SM16 ? NV / 2 : 1); ++i) asm volatile("" : "+r"(ohi[i])::"memory");
 
   // ---- write O: (256*hi + lo - zv * rowsum) * out_scale.  Row sums: column d (tile NDT - 1, t == 0).
   float rs0 = (float)(int)olo[4 * (NDT - 1)], rs1 = (float)(int)olo[4 * (NDT - 1) + 2];

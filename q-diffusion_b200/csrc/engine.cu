@@ -736,7 +736,9 @@ bool attention_wg_eligible(const qd_attention_desc& d) {
 
 template <int DQ, int DV, bool QS, bool VS, bool S16, bool F16>
 int launch_attention_wg_inst(const qd_attention_desc& d, cudaStream_t s) {
-  auto kern = qd::qattention_wg_kernel<DQ, DV, QS, VS, S16, F16>;
+  // d <= 40 fits 128 registers without spills: two CTAs per SM (DESIGN §6); larger d would spill there
+  constexpr int MINB = DV <= 40 ? 2 : 1;
+  auto kern = qd::qattention_wg_kernel<DQ, DV, QS, VS, S16, F16, MINB>;
   const int P = d.head_stride_q;
   const qd::AtwSmem lay = qd::atw_smem(P, qd::atw_nv(DV));
   static std::atomic<unsigned long long> optin{0};
