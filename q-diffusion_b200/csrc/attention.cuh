@@ -146,6 +146,15 @@ __device__ __forceinline__ int att_smax(int a, int b) { return max(a, b); }
 __device__ __forceinline__ float att_smax(float a, float b) { return fmaxf(a, b); }
 __device__ __forceinline__ int att_lowest(int) { return INT_MIN; }
 __device__ __forceinline__ float att_lowest(float) { return -INFINITY; }
+// Score of a masked key (beyond Tk in the last key tile).  It is below every reachable score and its exponent
+// fmaf(att_s2f(mask), c, b) is -inf, so the key takes no part in the row maximum, the row sum or the P codes whatever the
+// codes are: -inf as an fp32 score (fp16 operands); on int32 scores converted by att_i2f<true> the integer that the
+// conversion turns into the bit pattern of -inf.  att_i2f<false> (d > 64) turns INT_MIN into -2^31 instead, at least
+// 2^31 - 255^2 d below every score: its probability is exactly 0 for the sim_scale values launch_attention accepts.
+template <bool MAGIC>
+__device__ __forceinline__ int att_mask(int) { return MAGIC ? (int)(0xFF800000u - 0x4B400000u) : INT_MIN; }
+template <bool MAGIC>
+__device__ __forceinline__ float att_mask(float) { return -INFINITY; }
 
 // DQ: reduction length of QK^T padded to a multiple of 32; DV: head dim d (multiple of 8).
 // Shared-memory tiles are addressed from the array symbol (the
@@ -289,11 +298,12 @@ qattention_kernel(const qd_attention_desc p) {
         }
       }
       if (ragged && tile == ntiles - 1) {
+        const SV mask = att_mask<MAGIC>(SV{});
 #pragma unroll
         for (int nt = 0; nt < 8; ++nt) {
           const int j = j0 + 8 * nt + 2 * t;
-          if (j >= p.Tk) { sacc[nt][0] = -(1 << 21); sacc[nt][2] = -(1 << 21); }
-          if (j + 1 >= p.Tk) { sacc[nt][1] = -(1 << 21); sacc[nt][3] = -(1 << 21); }
+          if (j >= p.Tk) { sacc[nt][0] = mask; sacc[nt][2] = mask; }
+          if (j + 1 >= p.Tk) { sacc[nt][1] = mask; sacc[nt][3] = mask; }
         }
       }
       if (pass == 0) {
@@ -497,8 +507,8 @@ qattention_smallk_kernel(const qd_attention_desc p, int slabs_per_warp) {
       const int2 z = *reinterpret_cast<const int2*>(sZrk + 8 * nt + 2 * t);
       sacc[nt][0] -= z.x; sacc[nt][1] -= z.y; sacc[nt][2] -= z.x; sacc[nt][3] -= z.y;
       const int j = 8 * nt + 2 * t;
-      if (j >= p.Tk) { sacc[nt][0] = -(1 << 21); sacc[nt][2] = -(1 << 21); }
-      if (j + 1 >= p.Tk) { sacc[nt][1] = -(1 << 21); sacc[nt][3] = -(1 << 21); }
+      if (j >= p.Tk) { sacc[nt][0] = att_mask<MAGIC>(0); sacc[nt][2] = att_mask<MAGIC>(0); }
+      if (j + 1 >= p.Tk) { sacc[nt][1] = att_mask<MAGIC>(0); sacc[nt][3] = att_mask<MAGIC>(0); }
     }
     // ---- row statistics (rows g and g+8; a row lives in the 4 lanes of a quad)
     int mi0 = sacc[0][0], mi1 = sacc[0][2];

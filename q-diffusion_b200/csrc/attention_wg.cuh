@@ -274,12 +274,15 @@ qattention_wg_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_const
 
   // ---- Q fragments (rows g, g+8 of this warp's 16-row slab) in the m16n8k32 / m16n8k16 A layout: bytes 4t.. and
   // 16+4t.. of every 32-byte k-chunk; zero beyond the head's row (the K tile may hold the next head's bytes there).
+  // At d = 48 (8-bit and fp16 operands alike) ptxas of CUDA 12.9 hands the registers of fragments that stay live across
+  // the key loop to the P fragments of the first PV wgmma, so every later S = Q K^T read P codes as Q: the kernel then
+  // loads the fragments again for every key tile (L1 hits), which keeps them out of the loop's live set.
+  constexpr bool QRELOAD = DV == 48;
   uint32_t qf[NKC][4];
-  {
-    const uint8_t* qbase = reinterpret_cast<const uint8_t*>(p.q) + (long long)b * p.Tq * p.ld_q + p.q_off + h * p.head_stride_q;
-    const int r0 = min(row0 + g, p.Tq - 1), r1 = min(row0 + g + 8, p.Tq - 1);
-    const uint8_t* q0 = qbase + (long long)r0 * p.ld_q;
-    const uint8_t* q1 = qbase + (long long)r1 * p.ld_q;
+  const uint8_t* qbase = reinterpret_cast<const uint8_t*>(p.q) + (long long)b * p.Tq * p.ld_q + p.q_off + h * p.head_stride_q;
+  const uint8_t* q0 = qbase + (long long)min(row0 + g, p.Tq - 1) * p.ld_q;
+  const uint8_t* q1 = qbase + (long long)min(row0 + g + 8, p.Tq - 1) * p.ld_q;
+  auto load_q = [&]() {
 #pragma unroll
     for (int kc = 0; kc < NKC; ++kc) {
       const int c0 = kc * 32 + 4 * t, c1 = c0 + 16;
@@ -288,7 +291,8 @@ qattention_wg_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_const
       qf[kc][2] = c1 < RB ? *reinterpret_cast<const uint32_t*>(q0 + c1) : 0u;
       qf[kc][3] = c1 < RB ? *reinterpret_cast<const uint32_t*>(q1 + c1) : 0u;
     }
-  }
+  };
+  if constexpr (!QRELOAD) load_q();
   const float c = p.sim_scale * 1.4426950408889634f;
   const bool ragged = (p.Tk % ATT_BN) != 0;
   SV mi0 = att_lowest(SV{}), mi1 = att_lowest(SV{});
@@ -302,6 +306,7 @@ qattention_wg_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_const
   // (m16n8 fragments)
   auto issue_s = [&](SV (&s)[8][4], int L) {
     const int st = L % ATW_STAGES;
+    if constexpr (QRELOAD) load_q();
     mbar_wait(&full[st], (uint32_t)(L / ATW_STAGES) & 1u);
     const uint64_t dK = atw_desc(smem_u32(smem + st * lay.k_bytes), P);
     wgmma_fence();
@@ -349,11 +354,12 @@ qattention_wg_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_const
       }
     }
     if (ragged && tile == ntiles - 1) {
+      const SV mask = att_mask<MAGIC>(SV{});
 #pragma unroll
       for (int nt = 0; nt < 8; ++nt) {
         const int j = j0 + 8 * nt + 2 * t;
-        if (j >= p.Tk) { sacc[nt][0] = -(1 << 21); sacc[nt][2] = -(1 << 21); }
-        if (j + 1 >= p.Tk) { sacc[nt][1] = -(1 << 21); sacc[nt][3] = -(1 << 21); }
+        if (j >= p.Tk) { sacc[nt][0] = mask; sacc[nt][2] = mask; }
+        if (j + 1 >= p.Tk) { sacc[nt][1] = mask; sacc[nt][3] = mask; }
       }
     }
     if (pass == 0) {

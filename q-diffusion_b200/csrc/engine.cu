@@ -724,9 +724,6 @@ bool attention_wg_eligible(const qd_attention_desc& d) {
   const int P = d.head_stride_q, rb = d.qk_f16 ? 2 * d.d : d.d;
   if (d.d != 16 && d.d != 24 && d.d != 32 && d.d != 40 && d.d != 48 && d.d != 64 && d.d != 80 && d.d != 96) return false;
   if (d.qk_f16 && d.d > 64) return false;
-  // fp16 Q / K at d = 48 (LSUN-church 16x16 level) diverges from the oracle on this kernel, cause not found yet: it keeps the
-  // mma.sync kernel, which matches it
-  if (d.qk_f16 && d.d == 48) return false;
   if ((P != 32 && P != 64 && P != 128) || P < rb || d.head_stride_k != P) return false;
   if (d.q_off != 0 || d.k_off != 0 || (d.ld_k & 15) || (((uintptr_t)d.k) & 15) || (((uintptr_t)d.vt) & 15)) return false;
   if (d.v_off != 0 || d.head_stride_v != d.d || d.v_batch_stride != (long long)d.heads * d.d * d.ld_vt) return false;
@@ -805,6 +802,12 @@ int launch_attention(const qd_attention_desc& d, cudaStream_t s) {
   if (d.q_signed != d.k_signed) return fail(QD_ERR_UNSUPPORTED, "attention: q/k signedness differ");
   if (d.zw != 0) return fail(QD_ERR_UNSUPPORTED, "attention: softmax zero point must be 0 (got %d)", d.zw);
   if (d.sm_bits != 8 && d.sm_bits != 16) return fail(QD_ERR_UNSUPPORTED, "attention: sm_bits %d", d.sm_bits);
+  // Keys beyond Tk get the score att_mask (attention.cuh).  On int32 scores at d > 64 that is INT_MIN, whose exponent lies
+  // at least (2^31 - 255^2 d) * c below the row maximum's: ex2 flushes it to 0 once that exceeds 127 plus log2(1 / delta_w).
+  if (!(d.sim_scale > 0.f)) return fail(QD_ERR_UNSUPPORTED, "attention: sim_scale must be positive (got %g)", d.sim_scale);
+  if (!d.qk_f16 && d.d > 64 &&
+      (2147483648.0 - 65025.0 * d.d) * d.sim_scale * 1.4426950408889634 < 128.0 + fmax(0.0, -log2((double)d.delta_w)))
+    return fail(QD_ERR_UNSUPPORTED, "attention: sim_scale %g too small to mask the keys beyond Tk at d = %d", d.sim_scale, d.d);
   if (d.ld_vt % 16 || d.ld_vt < d.Tk) return fail(QD_ERR_BAD_ARG, "attention: ld_vt");
   if ((d.q_off | d.head_stride_q | (int)d.ld_q) & 3) return fail(QD_ERR_UNSUPPORTED, "attention: q needs 4-byte alignment");
   if ((d.k_off | d.head_stride_k | (int)d.ld_k | d.d) & 7) return fail(QD_ERR_UNSUPPORTED, "attention: k rows need 8-byte alignment");

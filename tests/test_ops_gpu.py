@@ -453,8 +453,6 @@ def test_im2col(cuda, stride, pad_tl, pad_total, C):
 
 def _run_attention(cuda, B, heads, d, Tq, Tk, sym, sm_bits, seed, f16=False):
     """q,k,v float -> codes (oracle quantizer) -> kernel; oracle = fake-quant attention on the same floats."""
-    ops, _ = _ops()
-    from qdiff_b200._lib import AttentionDesc, ptr
     gen = torch.Generator().manual_seed(seed)
     q = torch.randn(B, Tq, heads * d, generator=gen) * 1.5
     k = torch.randn(B, Tk, heads * d, generator=gen) * 1.5
@@ -475,51 +473,93 @@ def _run_attention(cuda, B, heads, d, Tq, Tk, sym, sm_bits, seed, f16=False):
                                  scale)
     ref = ref.reshape(B, heads, Tq, d).permute(0, 2, 1, 3).reshape(B, Tq, heads * d)
 
+    def codes(t, T, qp):
+        return O.uaq_codes(t, *qp).reshape(B, T, heads, d).to(torch.int32)
+
+    out = attention_codes(cuda, codes(q, Tq, qp_q), codes(k, Tk, qp_k), codes(v, Tk, qp_v), (qp_q[1], qp_k[1], qp_v[1]),
+                          sym, sm_bits, qp_q[0] * qp_k[0] * scale, dw, qp_v[0], f16=f16)
+    return out, ref
+
+
+def attention_codes(cuda, qc, kc, vc, zp, sym, sm_bits, sim_scale, dw, dv, *, f16=False, layout="padded", oq=None,
+                    junk=None):
+    """One qd_qattention call on integer codes: qc [B, Tq, heads, d], kc / vc [B, Tk, heads, d], zero points
+    zp = (zq, zk, zv); s8 codes if sym, else u8.  The softmax quantizer has step dw, zero point 0 and sm_bits bits; the
+    output step is dw * dv.
+    layout "padded": Q / K in the per-head padded layout the to_q / to_k GEMMs write (pitch 32 / 64 / 128 bytes, d beyond
+    112), dense V^T; "offset": Q / K heads packed at pitch d (2 d bytes in fp16) behind an 8-byte column offset and V^T
+    behind 8 leading rows, a layout only the mma.sync kernel takes.  f16: Q / K as fp16 centred codes (qk_f16).
+    junk: a torch.Generator that fills every byte the kernel must ignore (pitch padding, the column offset, V^T rows
+    before v_off and keys Tk .. ld_vt) with random codes instead of zeros.
+    oq: the consumer's activation quantizer (ops.act_qparams); the kernel then writes its codes (out_q) instead of fp32.
+    Returns the fp32 output or the codes, [B, Tq, heads * d], on the CPU."""
+    ops, _ = _ops()
+    from qdiff_b200._lib import AttentionDesc, ptr
+    B, Tq, heads, d = qc.shape
+    Tk = kc.shape[1]
     dt = torch.int8 if sym else torch.uint8
-    P = 32 if d <= 32 else 64 if d <= 64 else 128 if d <= 112 else d     # per-head pitch of the code layout
+    lo, hi = (-128, 127) if sym else (0, 255)
+    es = 2 if f16 else 1          # bytes per Q / K element; the descriptor counts bytes
+    if layout == "padded":
+        if f16:      # the swizzle span holding 2 * d bytes
+            P = 32 if d <= 16 else 64 if d <= 32 else 128
+        else:
+            P = 32 if d <= 32 else 64 if d <= 64 else 128 if d <= 112 else d
+        off, voff = 0, 0
+    else:
+        assert layout == "offset", layout
+        P, off, voff = es * d, 8, 8
 
-    def padded(t, T, zp=0):
-        if f16:      # qk_f16 operands: fp16 (code - zero_point), pitch in BYTES = the swizzle span holding 2 * d
-            out = torch.zeros(B, T, heads, P // 2, dtype=torch.float16)
-            out[..., :d] = (t.reshape(B, T, heads, d).to(torch.int32) - zp).to(torch.float16)
-            return out.reshape(B, T, heads * (P // 2)).to(cuda)
-        out = torch.zeros(B, T, heads, P, dtype=dt)
-        out[..., :d] = t.reshape(B, T, heads, d).to(dt)
-        return out.reshape(B, T, heads * P).to(cuda)
+    def fill(shape, dtype):
+        if junk is None:
+            return torch.zeros(shape, dtype=dtype)
+        if dtype == torch.float16:
+            return torch.randint(-255, 256, shape, generator=junk).to(dtype)
+        return torch.randint(lo, hi + 1, shape, generator=junk).to(dtype)
 
-    if f16:
-        P = 32 if d <= 16 else 64 if d <= 32 else 128
-    qc = padded(O.uaq_codes(q, *qp_q), Tq, qp_q[1])
-    kc = padded(O.uaq_codes(k, *qp_k), Tk, qp_k[1])
-    vc = O.uaq_codes(v, *qp_v).to(dt)
+    def qk_rows(c, z):
+        T = c.shape[1]
+        ld = (off + heads * P + 15) // 16 * 16       # bytes per row
+        buf = fill((B, T, ld // es), torch.float16 if f16 else dt)
+        body = buf[:, :, off // es:(off + heads * P) // es].unflatten(-1, (heads, P // es))
+        body[..., :d] = (c - z).to(torch.float16) if f16 else c.to(dt)
+        return buf.to(cuda), ld
+
+    qbuf, ld_q = qk_rows(qc, zp[0])
+    kbuf, ld_k = qk_rows(kc, zp[1])
     Tk_pad = (Tk + 15) // 16 * 16
-    vt = torch.zeros(B, heads * d, Tk_pad, dtype=dt)
+    vt = fill((B, voff + heads * d, Tk_pad), dt)
     tt = torch.arange(Tk)
     pos = (tt & ~15) | (((tt >> 1) & 3) << 2) | (((tt >> 3) & 1) << 1) | (tt & 1)   # att_vt_perm
-    vt[:, :, pos] = vc.permute(0, 2, 1)
+    vt[:, voff:, pos] = vc.reshape(B, Tk, heads * d).permute(0, 2, 1).to(dt)
     vt = vt.to(cuda)
     ws = torch.zeros(B * heads * ((Tk + 127) // 128 * 128), dtype=torch.int32, device=cuda)
-    out = torch.full((B, Tq, heads * d), float("nan"), device=cuda)
     a = AttentionDesc()
-    a.q, a.k, a.vt = ptr(qc), ptr(kc), ptr(vt)
-    a.ld_q = a.ld_k = heads * P
-    a.ld_vt, a.v_batch_stride = Tk_pad, heads * d * Tk_pad
+    a.q, a.k, a.vt = ptr(qbuf), ptr(kbuf), ptr(vt)
+    a.ld_q, a.ld_k = ld_q, ld_k
+    a.ld_vt, a.v_batch_stride = Tk_pad, (voff + heads * d) * Tk_pad
     a.B, a.heads, a.d, a.Tq, a.Tk = B, heads, d, Tq, Tk
-    a.q_off = a.k_off = a.v_off = 0
+    a.q_off = a.k_off = off
+    a.v_off = voff
     a.head_stride_q = a.head_stride_k = P
     a.head_stride_v = d
     a.q_signed = a.k_signed = a.v_signed = 1 if sym else 0
-    a.zq, a.zk, a.zv, a.zw = qp_q[1], qp_k[1], qp_v[1], 0
+    a.zq, a.zk, a.zv, a.zw = zp[0], zp[1], zp[2], 0
     a.p_qmin, a.p_qmax, a.sm_bits = 0, 2 ** sm_bits - 1, sm_bits
-    a.sim_scale = qp_q[0] * qp_k[0] * scale
+    a.sim_scale = sim_scale
     a.delta_w = dw
-    a.out_scale = dw * qp_v[0]
-    a.out, a.ld_out = ptr(out), heads * d
+    a.out_scale = dw * dv
+    if oq is None:
+        out = torch.full((B, Tq, heads * d), float("nan"), device=cuda)
+        a.out, a.ld_out = ptr(out), heads * d
+    else:
+        out = torch.zeros(B, Tq, heads * d, dtype=torch.int8 if oq.qmin < 0 else torch.uint8, device=cuda)
+        a.out_q, a.ld_out_q, a.oq = ptr(out), heads * d, oq
     a.ws = ptr(ws)
     a.qk_f16 = 1 if f16 else 0
     ops.attention(a)
     torch.cuda.synchronize()
-    return out.cpu(), ref
+    return out.cpu()
 
 
 @pytest.mark.parametrize("B,heads,d,Tq,Tk,sym,sm_bits", [
