@@ -80,7 +80,7 @@ typedef struct qd_gemm_desc {
   void* out_q;           /* codes or NULL */
   long long ldq;
   qd_qparams oq;
-  int32_t bn_hint;       /* 0 = auto N-tile */
+  int32_t bn_hint;       /* 0 = auto N-tile; else the N tile: a multiple of 16 up to 128 (geglu: of 32) */
   int32_t out_q_head_dim;   /* > 0: row-major out_q is written per head with padding: column n -> */
   int32_t out_q_head_pitch; /*      (n / head_dim) * head_pitch + n % head_dim   (attention Q / K operands) */
   int32_t geglu;         /* 1: rows of w (and scale/bias/corr) are interleaved [4 x-features, 4 gate-features]...;

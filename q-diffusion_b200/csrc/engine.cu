@@ -221,6 +221,10 @@ int plan_gemm(const qd_gemm_desc* d, GemmPlan* pl) {
       return fail(QD_ERR_BAD_ARG, "gemm: geglu needs N %% 8 == 0, out_q only, plain GEMM");
   }
   a.BN = pick_bn(d->N, a.tiles_m, sms, d->bn_hint, d->geglu ? 32 : 16, (long long)d->C * d->taps * a.kdup);
+  // the GEGLU epilogue finalises whole 32-column chunks (4 x 8 interleaved x / gate columns): a narrower last chunk would
+  // read accumulator columns the tile never wrote and store codes into the next N tile's output columns
+  if (d->geglu && (a.BN % 32))
+    return fail(QD_ERR_BAD_ARG, "gemm: geglu needs an N tile that is a multiple of 32 (bn_hint %d)", d->bn_hint);
   const int bn_default = a.BN;
   // split-K candidates (see below) take the widest N tile: few tiles remain, and what is shared among the SMs is the K loop
   // (the split-K partial kernel takes up to qd::GEMM_MAX_BN_SPLITK columns; without split-K the tile reverts to bn_default)
