@@ -195,8 +195,14 @@ int qd_groupnorm_quant(const qd_groupnorm_desc* d, qd_stream_t stream);
  * qd_attention_fp32 -- softmax(scale * q k^T) v per (batch, head) in fp32: QuantAttnBlock.forward with use_act_quant
  *   False (qdiff/quant_block.py:360-386) and QKVAttentionLegacy (openaimodel.py:384-406; scale = 1/sqrt(ch) applied to
  *   the product).  q: [B*Tq, ld_q], head h at columns q_off + h*head_stride_q (k, v likewise); out [B*Tq, ld_out].
+ *   causal = 1: query row r attends to keys 0..r only (the CLIP text encoder's self-attention, CLIPAttention.forward of
+ *   transformers' modeling_clip.py with the causal mask of CLIPTextTransformer: FrozenCLIPEmbedder.forward,
+ *   ldm/modules/encoders/modules.py:150-155).  Masked keys take no probability whatever their values.  Needs Tq == Tk;
+ *   always runs the one-row-per-block kernel.  0 (what a zero-initialised descriptor holds): every key.
  * ------------------------------------------------------------------------------------------ */
-/* qd_split_desc.act: 0 none, 1 SiLU, 2 GEGLU (src has 2*C columns: value = src[:, c] * gelu_erf(src[:, C + c])) */
+/* qd_split_desc.act: 0 none, 1 SiLU, 2 GEGLU (src has 2*C columns: value = src[:, c] * gelu_erf(src[:, C + c])),
+ * 3 quick-GELU x * sigmoid(1.702 x) in fp32 with the accurate exponential (CLIPMLP with hidden_act "quick_gelu", the
+ * activation between fc1 and fc2 of the text encoder that FrozenCLIPEmbedder runs, modules.py:150-155) */
 typedef struct qd_split_desc {
   const float* src;
   long long ld_src;
@@ -218,7 +224,24 @@ typedef struct qd_attention_fp_desc {
   float scale;
   float* out;
   long long ld_out;
+  int32_t causal;        /* 0: all Tk keys; 1: key j <= query row r only (Tq == Tk) */
 } qd_attention_fp_desc;
+
+/* qd_embed_tokens -- the text encoder's input embedding (CLIPTextEmbeddings.forward of transformers' modeling_clip.py,
+ *   called by FrozenCLIPEmbedder.forward, ldm/modules/encoders/modules.py:150-155):
+ *   out[(b*T + t) * ld_out + c] = tok[ids[b*T + t] * C + c] + pos[t * C + c]   (fp32, one rounding: torch's add)
+ *   ids int32 [B*T]; tok [vocab][C], pos [>= T][C] fp32.  An id outside [0, vocab) writes NaN across its row (the host
+ *   refuses such ids before they are uploaded). */
+typedef struct qd_embed_desc {
+  const int32_t* ids;
+  const float* tok;
+  const float* pos;
+  float* out;
+  long long ld_out;
+  int32_t B, T, C, vocab;
+} qd_embed_desc;
+
+int qd_embed_tokens(const qd_embed_desc* d, qd_stream_t stream);
 
 /* out[i] = a*x[i] + b*y[i] + c*z[i] (y / z may be NULL): the DPM-Solver++ multistep update
  * x_t = (sigma_t/sigma_s) x - alpha_t (e^-h - 1) m0 - 0.5 alpha_t (e^-h - 1) D1   (dpm_solver.py:504-527, 755-795). */
@@ -411,7 +434,8 @@ enum qd_op_kind {
   QD_OP_SPLIT3 = 13,
   QD_OP_ATTENTION_FP = 14,
   QD_OP_VQ_LOOKUP = 15,
-  QD_OP_SOFTMAX_ROWS = 16
+  QD_OP_SOFTMAX_ROWS = 16,
+  QD_OP_EMBED = 17        /* desc: qd_embed_desc */
 };
 
 /* generic argument block for the small helpers when recorded into an engine */
@@ -425,7 +449,7 @@ typedef struct qd_misc_desc {
 } qd_misc_desc;
 
 int qd_engine_create(int device, qd_engine** out);
-/* desc points at the matching qd_*_desc (qd_misc_desc for kinds >= 7); copied. */
+/* desc points at the matching qd_*_desc (qd_misc_desc for kinds 7..12, 15, 16; qd_embed_desc for QD_OP_EMBED); copied. */
 int qd_engine_add_op(qd_engine* e, int kind, const void* desc);
 int qd_engine_num_ops(const qd_engine* e);
 int qd_engine_finalize(qd_engine* e);

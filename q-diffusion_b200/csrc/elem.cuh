@@ -16,6 +16,9 @@ __device__ __forceinline__ uint32_t pack4(uint32_t a, uint32_t b, uint32_t c, ui
 }
 __device__ __forceinline__ float silu_f(float x) { return silu_fast(x); }
 __device__ __forceinline__ float gelu_erf_f(float x) { return 0.5f * x * (1.0f + erff(x * 0.70710678118654752440f)); }
+// quick_gelu of transformers' activations.py (x * sigmoid(1.702 x)), the CLIP text encoder's MLP activation; expf, not
+// __expf: the weight-only planes carry the value to 2^-24
+__device__ __forceinline__ float quick_gelu_f(float x) { return x * (1.0f / (1.0f + expf(-1.702f * x))); }
 
 // ------------------------------------------------------------------------------------ quantize
 // One thread = 4 consecutive channels of one row.
@@ -109,6 +112,7 @@ __global__ void split_bf16x3_kernel(const qd_split_desc p) {
     for (int j = 0; j < 4; ++j) {
       float x = v[j];
       if (p.act == 1) x = x / (1.0f + __expf(-x));          // SiLU with the accurate exponential (this path is fp32-faithful)
+      else if (p.act == 3) x = quick_gelu_f(x);
       const float h = bf16_rn(x);
       const float r1 = x - h;
       const float m = bf16_rn(r1);
@@ -133,6 +137,7 @@ __global__ void split_bf16x3_scalar_kernel(const qd_split_desc p) {
     float x = p.src[r * p.ld_src + c];
     if (p.act == 1) x = x / (1.0f + __expf(-x));
     else if (p.act == 2) x *= gelu_erf_f(p.src[r * p.ld_src + p.C + c]);
+    else if (p.act == 3) x = quick_gelu_f(x);
     const float h = bf16_rn(x);
     const float r1 = x - h;
     const float m = bf16_rn(r1);
@@ -154,11 +159,13 @@ __global__ void __launch_bounds__(128) attention_fp32_kernel(const qd_attention_
   __shared__ float red[4];
   const int bh = blockIdx.y, b = bh / p.heads, h = bh - b * p.heads;
   const int r = blockIdx.x;
+  // causal: keys r+1.. are never read, so they take no probability whatever they hold (the launcher checks Tq == Tk)
+  const int nk = p.causal ? min(r + 1, p.Tk) : p.Tk;
   const float* q = p.q + ((long long)b * p.Tq + r) * p.ld_q + p.q_off + h * p.head_stride_q;
   for (int i = threadIdx.x; i < p.d; i += blockDim.x) qs[i] = q[i];
   __syncthreads();
   float mx = -INFINITY;
-  for (int j = threadIdx.x; j < p.Tk; j += blockDim.x) {
+  for (int j = threadIdx.x; j < nk; j += blockDim.x) {
     const float* k = p.k + ((long long)b * p.Tk + j) * p.ld_k + p.k_off + h * p.head_stride_k;
     float acc = 0.f;
     for (int i = 0; i < p.d; ++i) acc = fmaf(qs[i], k[i], acc);
@@ -172,7 +179,7 @@ __global__ void __launch_bounds__(128) attention_fp32_kernel(const qd_attention_
   mx = fmaxf(fmaxf(red[0], red[1]), fmaxf(red[2], red[3]));
   __syncthreads();
   float sum = 0.f;
-  for (int j = threadIdx.x; j < p.Tk; j += blockDim.x) {
+  for (int j = threadIdx.x; j < nk; j += blockDim.x) {
     const float e = expf(sc[j] - mx);
     sc[j] = e;
     sum += e;
@@ -185,8 +192,22 @@ __global__ void __launch_bounds__(128) attention_fp32_kernel(const qd_attention_
   for (int c = threadIdx.x; c < p.d; c += blockDim.x) {
     const float* v = p.v + (long long)b * p.Tk * p.ld_v + p.v_off + h * p.head_stride_v + c;
     float acc = 0.f;
-    for (int j = 0; j < p.Tk; ++j) acc = fmaf(sc[j] * inv, v[(long long)j * p.ld_v], acc);
+    for (int j = 0; j < nk; ++j) acc = fmaf(sc[j] * inv, v[(long long)j * p.ld_v], acc);
     o[c] = acc;
+  }
+}
+
+// ------------------------------------------------------------------------------------ text encoder input embedding
+// out[b*T + t] = tok[ids[b, t]] + pos[t] (CLIPTextEmbeddings.forward): one thread per channel, rows over the grid
+__global__ void embed_tokens_kernel(const qd_embed_desc p) {
+  const long long total = (long long)p.B * p.T * p.C;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
+    const long long row = i / p.C;
+    const int c = (int)(i - row * p.C);
+    const int t = (int)(row % p.T);
+    const int id = p.ids[row];
+    p.out[row * p.ld_out + c] = (id >= 0 && id < p.vocab) ? p.tok[(long long)id * p.C + c] + p.pos[(long long)t * p.C + c]
+                                                          : __int_as_float(0x7fc00000);
   }
 }
 

@@ -638,11 +638,13 @@ int launch_split3(const qd_split_desc& d, cudaStream_t s) {
 int launch_attention_fp(const qd_attention_fp_desc& d, cudaStream_t s) {
   if (!d.q || !d.k || !d.v || !d.out || d.B <= 0 || d.heads <= 0 || d.d <= 0 || d.Tq <= 0 || d.Tk <= 0)
     return fail(QD_ERR_BAD_ARG, "attention_fp32: bad args");
-  // long sequences: AFP_R query rows per block share the K / V rows they read (K/V traffic / AFP_R)
+  if (d.causal != 0 && d.causal != 1) return fail(QD_ERR_BAD_ARG, "attention_fp32: causal must be 0 or 1 (got %d)", d.causal);
+  if (d.causal && d.Tq != d.Tk) return fail(QD_ERR_UNSUPPORTED, "attention_fp32: causal needs Tq == Tk (got %d, %d)", d.Tq, d.Tk);
+  // long sequences (never causal: the text encoder's T = 77 takes the one-row kernel): AFP_R query rows per block share the K / V rows they read (K/V traffic / AFP_R)
   const size_t smem_rows = (size_t)qd::AFP_R * (d.d + qd::afp_tk_pitch(d.Tk)) * sizeof(float);
   const bool aligned = !(d.d & 3) && !(d.ld_q & 3) && !(d.ld_k & 3) && !(d.q_off & 3) && !(d.k_off & 3) && !(d.head_stride_q & 3) &&
                        !(d.head_stride_k & 3) && !((uintptr_t)d.q & 15) && !((uintptr_t)d.k & 15);
-  if (d.Tq >= 256 && smem_rows <= 200 * 1024 && aligned) {
+  if (!d.causal && d.Tq >= 256 && smem_rows <= 200 * 1024 && aligned) {
     static std::atomic<unsigned long long> optin{0};
     if (int rc = ensure_smem_optin(qd::attention_fp32_rows_kernel, 200 * 1024, optin, "attention_fp32_rows")) return rc;
     launch_k(qd::attention_fp32_rows_kernel, dim3((d.Tq + qd::AFP_R - 1) / qd::AFP_R, d.B * d.heads), 256, smem_rows, s, d);
@@ -652,6 +654,13 @@ int launch_attention_fp(const qd_attention_fp_desc& d, cudaStream_t s) {
   if (smem > 48 * 1024) return fail(QD_ERR_UNSUPPORTED, "attention_fp32: d + Tk = %d exceeds 12288 floats of shared memory", d.d + d.Tk);
   launch_k(qd::attention_fp32_kernel, dim3(d.Tq, d.B * d.heads), 128, smem, s, d);
   return check_launch("attention_fp32_kernel");
+}
+
+int launch_embed(const qd_embed_desc& d, cudaStream_t s) {
+  if (!d.ids || !d.tok || !d.pos || !d.out || d.B <= 0 || d.T <= 0 || d.C <= 0 || d.vocab <= 0 || d.ld_out < d.C)
+    return fail(QD_ERR_BAD_ARG, "embed_tokens: bad args (B=%d T=%d C=%d vocab=%d ld_out=%lld)", d.B, d.T, d.C, d.vocab, d.ld_out);
+  launch_k(qd::embed_tokens_kernel, grid_for((long long)d.B * d.T * d.C, 256), 256, 0, s, d);
+  return check_launch("embed_tokens_kernel");
 }
 
 int launch_im2col(const qd_im2col_desc& d, cudaStream_t s) {
@@ -898,6 +907,7 @@ struct Op {
     qd_misc_desc misc;
     qd_split_desc split;
     qd_attention_fp_desc attfp;
+    qd_embed_desc embed;
   };
   Op() : kind(0) { memset(&gemm, 0, sizeof(gemm)); memset(&gn, 0, sizeof(gn)); }
 };
@@ -912,6 +922,7 @@ int run_op(const Op& op, cudaStream_t s) {
     case QD_OP_ATTENTION: return launch_attention(op.att, s);
     case QD_OP_SPLIT3: return launch_split3(op.split, s);
     case QD_OP_ATTENTION_FP: return launch_attention_fp(op.attfp, s);
+    case QD_OP_EMBED: return launch_embed(op.embed, s);
     default: return launch_misc(op.kind, op.misc, s);
   }
 }
@@ -974,6 +985,10 @@ int qd_split_bf16x3(const qd_split_desc* d, qd_stream_t s) {
 int qd_attention_fp32(const qd_attention_fp_desc* d, qd_stream_t s) {
   if (!d) return fail(QD_ERR_BAD_ARG, "null desc");
   return launch_attention_fp(*d, (cudaStream_t)s);
+}
+int qd_embed_tokens(const qd_embed_desc* d, qd_stream_t s) {
+  if (!d) return fail(QD_ERR_BAD_ARG, "null desc");
+  return launch_embed(*d, (cudaStream_t)s);
 }
 int qd_timestep_embedding(const float* t, const float* freqs, int32_t B, int32_t dim, int32_t mode, float* out,
                           qd_stream_t s) {
@@ -1054,6 +1069,7 @@ int qd_engine_add_op(qd_engine* e, int kind, const void* desc) {
     case QD_OP_ATTENTION: op.att = *reinterpret_cast<const qd_attention_desc*>(desc); break;
     case QD_OP_SPLIT3: op.split = *reinterpret_cast<const qd_split_desc*>(desc); break;
     case QD_OP_ATTENTION_FP: op.attfp = *reinterpret_cast<const qd_attention_fp_desc*>(desc); break;
+    case QD_OP_EMBED: op.embed = *reinterpret_cast<const qd_embed_desc*>(desc); break;
     case QD_OP_TIMESTEP_EMB: case QD_OP_COPY2D: case QD_OP_NCHW_TO_NHWC: case QD_OP_NHWC_TO_NCHW:
     case QD_OP_AVGPOOL2X: case QD_OP_UPSAMPLE2X: case QD_OP_VQ_LOOKUP: case QD_OP_SOFTMAX_ROWS:
       op.misc = *reinterpret_cast<const qd_misc_desc*>(desc);

@@ -18,7 +18,7 @@ c_vp = C.c_void_p
 
 QD_OP_GEMM, QD_OP_QUANTIZE, QD_OP_GROUPNORM, QD_OP_LAYERNORM, QD_OP_IM2COL, QD_OP_ATTENTION = 1, 2, 3, 4, 5, 6
 QD_OP_TIMESTEP_EMB, QD_OP_COPY2D, QD_OP_NCHW_TO_NHWC, QD_OP_NHWC_TO_NCHW, QD_OP_AVGPOOL2X, QD_OP_UPSAMPLE2X = 7, 8, 9, 10, 11, 12
-QD_OP_SPLIT3, QD_OP_ATTENTION_FP, QD_OP_VQ_LOOKUP, QD_OP_SOFTMAX_ROWS = 13, 14, 15, 16
+QD_OP_SPLIT3, QD_OP_ATTENTION_FP, QD_OP_VQ_LOOKUP, QD_OP_SOFTMAX_ROWS, QD_OP_EMBED = 13, 14, 15, 16, 17
 
 
 class QParams(C.Structure):
@@ -114,7 +114,12 @@ class AttentionFpDesc(C.Structure):
                 ("B", c_i32), ("heads", c_i32), ("d", c_i32), ("Tq", c_i32), ("Tk", c_i32),
                 ("q_off", c_i32), ("k_off", c_i32), ("v_off", c_i32),
                 ("head_stride_q", c_i32), ("head_stride_k", c_i32), ("head_stride_v", c_i32),
-                ("scale", c_f), ("out", c_vp), ("ld_out", c_ll)]
+                ("scale", c_f), ("out", c_vp), ("ld_out", c_ll), ("causal", c_i32)]
+
+
+class EmbedDesc(C.Structure):
+    _fields_ = [("ids", c_vp), ("tok", c_vp), ("pos", c_vp), ("out", c_vp), ("ld_out", c_ll),
+                ("B", c_i32), ("T", c_i32), ("C", c_i32), ("vocab", c_i32)]
 
 
 class MiscDesc(C.Structure):
@@ -141,7 +146,7 @@ class AncestralDesc(C.Structure):
 
 EXPORTS = [
     "qd_qgemm_i8", "qd_quantize", "qd_groupnorm_quant", "qd_groupnorm_workspace_floats", "qd_layernorm_quant",
-    "qd_im2col_i8", "qd_qattention", "qd_split_bf16x3", "qd_attention_fp32", "qd_lincomb3", "qd_timestep_embedding", "qd_copy2d", "qd_nchw_to_nhwc", "qd_nhwc_to_nchw", "qd_avgpool2x", "qd_upsample2x_f32", "qd_vq_lookup", "qd_softmax_rows",
+    "qd_im2col_i8", "qd_qattention", "qd_split_bf16x3", "qd_attention_fp32", "qd_embed_tokens", "qd_lincomb3", "qd_timestep_embedding", "qd_copy2d", "qd_nchw_to_nhwc", "qd_nhwc_to_nchw", "qd_avgpool2x", "qd_upsample2x_f32", "qd_vq_lookup", "qd_softmax_rows",
     "qd_sampler_step", "qd_ancestral_step", "qd_engine_create", "qd_engine_add_op", "qd_engine_num_ops", "qd_engine_finalize",
     "qd_engine_run", "qd_engine_run_range", "qd_engine_destroy", "qd_last_error", "qd_num_sms", "qd_launch_count",
 ]
@@ -164,7 +169,8 @@ def lib():
     L.qd_last_error.restype = C.c_char_p
     L.qd_launch_count.restype = c_ll
     for name in ("qd_qgemm_i8", "qd_quantize", "qd_groupnorm_quant", "qd_layernorm_quant", "qd_im2col_i8",
-                 "qd_qattention", "qd_sampler_step", "qd_ancestral_step", "qd_split_bf16x3", "qd_attention_fp32"):
+                 "qd_qattention", "qd_sampler_step", "qd_ancestral_step", "qd_split_bf16x3", "qd_attention_fp32",
+                 "qd_embed_tokens"):
         getattr(L, name).argtypes = [c_vp, c_vp]
         getattr(L, name).restype = C.c_int
     L.qd_timestep_embedding.argtypes = [c_vp, c_vp, c_i32, c_i32, c_i32, c_vp, c_vp]

@@ -10,13 +10,22 @@ DDIM (default), --dpm (DPM-Solver++ 2M) and -v (the 1000-step ancestral loop); t
 names the sampler and its NFE (UNet calls per image batch).  Scope (SURVEY section 8): the denoising loop on a
 calibrated checkpoint -- `--ptq --resume --cali_ckpt ckpt.pth` (the checkpoint the reference's calibration wrote; it
 carries the FP weights, the AdaRound parameters and the activation quantizers, SURVEY Appendix C, so no base checkpoint
-is needed).  Calibration itself (`--ptq` without `--resume`), `--resume_w` and the text encoder
-are outside the hot path: those flags parse, and the run stops with a message naming what to do instead.
+is needed).  Calibration itself (`--ptq` without `--resume`) and `--resume_w` are outside the hot path: those flags
+parse, and the run stops with a message naming what to do instead.
+
+txt2img prompts (--prompt, --from-file) are encoded by the CLIP text encoder ON THE ENGINE (qdiff_b200.text_encoder)
+when --ckpt names a file holding `cond_stage_model.transformer.*` (the SD checkpoint the reference loads): its weights
+are the ones the reference runs.  The tokenizer files come from --b200_tokenizer DIR or the local Hugging Face cache of
+the yaml's cond_stage_config version (openai/clip-vit-large-patch14); nothing is downloaded.  --b200_context takes
+precedence; with neither, a seeded N(0,1) context is used.
 
 Extra flags of this implementation (all prefixed so they cannot collide with future reference flags):
     --b200_synthetic NAME     seeded synthetic weights + the committed calibration fixture (offline runs, no checkpoint)
     --b200_context FILE       txt2img: pre-computed prompt embeddings {"c": [B,77,768], "uc": [1|B,77,768]} (torch.save);
-                              without it a seeded N(0,1) context is used, like the reference's own dummy calibration input
+                              without it (and without a text encoder in --ckpt) a seeded N(0,1) context is used, like the
+                              reference's own dummy calibration input
+    --b200_tokenizer DIR      txt2img: directory with the CLIP tokenizer's vocab.json + merges.txt (default: the local
+                              Hugging Face cache)
     --b200_out FILE           where to save the latents / images tensor (default: <logdir or outdir>/samples.pt)
     --b200_decode             LDM / txt2img: decode the final latents with the first stage ON THE ENGINE (qdiff_b200.first_stage;
                               ddpm.py:710-767) and save the images in [0, 1] next to the latents.  Weights: --b200_first_stage
@@ -153,7 +162,8 @@ def txt2img_parser():
              (("--running_stat",), dict(action="store_true")), (("--rs_sm_only",), dict(action="store_true")),
              _TAIL[0], _TAIL[1]])
     _add(p, _B200)
-    _add(p, [(("--b200_context",), dict(type=str, default=None, help="pre-computed prompt embeddings (see module docstring)"))])
+    _add(p, [(("--b200_context",), dict(type=str, default=None, help="pre-computed prompt embeddings (see module docstring)")),
+             (("--b200_tokenizer",), dict(type=str, default=None, help="CLIP tokenizer directory (vocab.json, merges.txt)"))])
     return p
 
 
@@ -468,15 +478,64 @@ def run_ldm(args):
 
 
 # ---------------------------------------------------------------------------------------------- txt2img
+def _text_encoder_state(args):
+    """The `cond_stage_model.transformer.*` entries of --ckpt, or None (no --ckpt file, or one without a text encoder).
+    --b200_context takes precedence."""
+    if args.b200_context or not args.ckpt or not os.path.isfile(args.ckpt):
+        return None
+    import torch
+    sd = torch.load(args.ckpt, map_location="cpu", weights_only=False)
+    sd = sd.get("state_dict", sd) if isinstance(sd, dict) else {}
+    enc = {k: v for k, v in sd.items() if k.startswith("cond_stage_model.transformer.")}
+    return enc or None
+
+
+def _prompt_batches(args):
+    """txt2img.py:497-508: --prompt repeated n_samples times, or the lines of --from-file in chunks of n_samples.  A
+    short last chunk is refused: the reference cannot sample it either (its [uc; c] concatenation, plms.py:187)."""
+    B = args.n_samples
+    if not args.from_file:
+        if args.prompt is None:
+            raise SystemExit("--prompt is empty")
+        return [B * [args.prompt]]
+    with open(args.from_file, "r") as f:
+        data = f.read().splitlines()
+    if not data or len(data) % B:
+        raise SystemExit(f"--from-file {args.from_file}: {len(data)} prompts is not a positive multiple of --n_samples {B} "
+                         f"(every batch holds n_samples prompts; pad or trim the file)")
+    return [data[i:i + B] for i in range(0, len(data), B)]
+
+
+def _text_encoder(args, enc_sd, cfg_params, context_dim, dev):
+    """FrozenCLIPEmbedder on the engine from the --ckpt entries; checks the yaml's cond stage (non-synthetic runs)."""
+    from . import text_encoder as TE
+    version = TE.DEFAULT_VERSION
+    if cfg_params is not None:
+        csc = cfg_params.get("cond_stage_config") or {}
+        if not str(csc.get("target", "")).endswith("FrozenCLIPEmbedder"):
+            raise SystemExit(f"cond_stage_config.target {csc.get('target')!r}: the engine's text encoder is FrozenCLIPEmbedder")
+        version = (csc.get("params") or {}).get("version", version)
+    try:
+        enc = TE.build_text_encoder(enc_sd, tokenizer_dir=args.b200_tokenizer, version=version)
+    except FileNotFoundError as e:
+        raise SystemExit(str(e))
+    if enc.width != context_dim:
+        raise SystemExit(f"text encoder width {enc.width} != the UNet's context_dim {context_dim}")
+    return enc.to(dev)
+
+
 def run_txt2img(args):
-    """The sampling loop of the reference's main() (:505-541) on the engine: PLMS / DDIM with classifier-free guidance.
-    Prompt embeddings come from --b200_context (the CLIP text encoder is outside the scope); saves the latents,
-    with --b200_decode also the decoded images."""
+    """The sampling loop of the reference's main() (:497-541) on the engine: PLMS / DDIM with classifier-free guidance.
+    Prompt embeddings: --b200_context, else the CLIP text encoder of --ckpt on the engine (--prompt / --from-file,
+    get_learned_conditioning per batch; batch j of iteration n starts from seed + 1 + n * batches + j), else a seeded
+    N(0,1) context.  Saves the latents, with --b200_decode also the decoded images."""
     import torch
     from . import dist as qdist, samplers, unet
     _require_resume(args)
     if not args.cond:
         raise SystemExit("txt2img needs --cond (the reference asserts the same)")
+    enc_sd = _text_encoder_state(args)
+    batches = _prompt_batches(args) if enc_sd is not None else [None]     # checked before any device work
     rank, world, dev = _setup(args.seed)
     if args.precision == "autocast" and rank == 0:
         print("note: the engine computes the integer form of the fp32 (--precision full) path; autocast only affects "
@@ -497,7 +556,12 @@ def run_txt2img(args):
     B = args.n_samples
     per = _shard(B, world)
     lo = rank * per
-    if args.b200_context:
+    encoder = None
+    if enc_sd is not None:
+        encoder = _text_encoder(args, enc_sd, None if args.b200_synthetic else cfg, ctx_shape[-1], dev)
+        if rank == 0:
+            print(f"prompts: CLIP text encoder on the engine ({len(batches)} batch(es) of {B})")
+    elif args.b200_context:
         emb = torch.load(args.b200_context, map_location="cpu")
         c_full, uc_full = emb["c"].float(), emb.get("uc")
         if c_full.shape[0] == 1:
@@ -506,25 +570,31 @@ def run_txt2img(args):
         g = torch.Generator().manual_seed(args.seed + 1)
         c_full = torch.randn(B, *ctx_shape, generator=g)
         uc_full = torch.randn(1, *ctx_shape, generator=g)
-    c = c_full[lo:lo + per].contiguous().to(dev)
-    uc = None
-    if args.scale != 1.0:
-        if uc_full is None:
-            raise SystemExit("--scale != 1 needs the empty-prompt embedding 'uc' in --b200_context")
-        uc = uc_full.float().expand(B, -1, -1)[lo:lo + per].contiguous().to(dev)
+    if encoder is None:
+        c = c_full[lo:lo + per].contiguous().to(dev)
+        uc = None
+        if args.scale != 1.0:
+            if uc_full is None:
+                raise SystemExit("--scale != 1 needs the empty-prompt embedding 'uc' in --b200_context")
+            uc = uc_full.float().expand(B, -1, -1)[lo:lo + per].contiguous().to(dev)
     shape = (args.C, args.H // args.f, args.W // args.f)
     start = None
     if args.fixed_code:
         (start,) = qdist.shard_like_single_process((B,) + shape, args.seed, rank, world)
-    outs, t0 = [], time.time()
+    outs, prompts_all, t0 = [], [], time.time()
     for n in range(args.n_iter):
-        x_T = start
-        if x_T is None:
-            (x_T,) = qdist.shard_like_single_process((B,) + shape, args.seed + 1 + n, rank, world)
-        z, _ = sampler.sample(S=args.ddim_steps, conditioning=c, batch_size=per, shape=shape, verbose=False,
-                              unconditional_guidance_scale=args.scale, unconditional_conditioning=uc, eta=args.ddim_eta,
-                              x_T=x_T)
-        outs.append(qdist.gather_latents(z, world))
+        for j, prompts in enumerate(batches):
+            if encoder is not None:     # every rank encodes the whole batch and keeps its slice (as with the noise)
+                uc = encoder.encode(B * [""])[lo:lo + per].contiguous() if args.scale != 1.0 else None
+                c = encoder.encode(list(prompts))[lo:lo + per].contiguous()
+                prompts_all += list(prompts)
+            x_T = start
+            if x_T is None:
+                (x_T,) = qdist.shard_like_single_process((B,) + shape, args.seed + 1 + n * len(batches) + j, rank, world)
+            z, _ = sampler.sample(S=args.ddim_steps, conditioning=c, batch_size=per, shape=shape, verbose=False,
+                                  unconditional_guidance_scale=args.scale, unconditional_conditioning=uc, eta=args.ddim_eta,
+                                  x_T=x_T)
+            outs.append(qdist.gather_latents(z, world))
     z = torch.cat(outs)
     torch.cuda.synchronize()
     dt = time.time() - t0
@@ -532,6 +602,8 @@ def run_txt2img(args):
         print(f"{z.shape[0]} latents {tuple(z.shape[1:])}, {args.ddim_steps} {'PLMS' if args.plms else 'DDIM'} steps, "
               f"scale {args.scale}: {dt:.2f} s -> {z.shape[0] / dt:.3f} images/s on {world} GPU(s)")
     meta = dict(kind="latents", steps=args.ddim_steps, scale=args.scale, prompt=args.prompt)
+    if encoder is not None:
+        meta["prompts"] = prompts_all           # the prompt of every image, in sample order
     if args.b200_decode and rank == 0:
         fs, sf = _first_stage(args, args.b200_synthetic, None if args.b200_synthetic else cfg, dev)
         t1 = time.time()

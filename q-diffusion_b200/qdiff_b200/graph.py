@@ -1375,7 +1375,7 @@ class WeightOnlyBuilder(Builder):
         _, out_f = self.groupnorm(x, norm, hw, [], silu, label, ss=ss, want_f32=True, ss_src=ss_src)
         return out_f
 
-    def attention_fp(self, q, k, v, *, heads, d, Tq, Tk, q_layout, k_layout, v_layout, scale, label):
+    def attention_fp(self, q, k, v, *, heads, d, Tq, Tk, q_layout, k_layout, v_layout, scale, label, causal=False):
         out = self.new_f32(self.B * Tq, heads * d)
         a = _lib.AttentionFpDesc()
         a.q, a.k, a.v = q.ptr, k.ptr, v.ptr
@@ -1386,9 +1386,10 @@ class WeightOnlyBuilder(Builder):
         a.v_off, a.head_stride_v = v_layout
         a.scale = float(scale)
         a.out, a.ld_out = out.ptr, out.ld
+        a.causal = 1 if causal else 0
         self.add(_lib.QD_OP_ATTENTION_FP, a, label, flops=4 * self.B * heads * Tq * Tk * d,
                  spec=dict(kind="attention_fp", q=q, k=k, v=v, B=self.B, heads=heads, d=d, Tq=Tq, Tk=Tk, q_layout=q_layout,
-                           k_layout=k_layout, v_layout=v_layout, scale=float(scale), out=out))
+                           k_layout=k_layout, v_layout=v_layout, scale=float(scale), out=out, causal=bool(causal)))
         return out
 
     # ------------------------------------------------------------------ shortcut convs (with or without split)

@@ -7,7 +7,8 @@ and scripts reach the UNet as model.model.diffusion_model (txt2img.py:367-383, D
 LatentDiffusionShim provides exactly that surface, so the reference's own sampler classes run unchanged on top of a
 qdiff_b200.QuantModel (tests/test_ldm_shim_cpu.py drives the reference's PLMSSampler / DDIMSampler over it), and so
 do this repo's samplers (qdiff_b200/samplers.py).  The first stage is optional (qdiff_b200.first_stage container:
-decode_first_stage runs on the engine, SURVEY section 8 f2); the cond stage (text encoder) is outside the scope.
+decode_first_stage runs on the engine, SURVEY section 8 f2), and so is the cond stage (qdiff_b200.text_encoder
+FrozenCLIPEmbedder: get_learned_conditioning runs the CLIP text encoder on the engine).
 """
 import numpy as np
 import torch
@@ -35,13 +36,14 @@ class DiffusionWrapper:
 
 class LatentDiffusionShim:
     def __init__(self, unet, conditioning_key=None, timesteps=1000, linear_start=1e-4, linear_end=2e-2,
-                 beta_schedule="linear", device=None, parameterization="eps", first_stage_model=None, scale_factor=1.0):
+                 beta_schedule="linear", device=None, parameterization="eps", first_stage_model=None, scale_factor=1.0,
+                 cond_stage_model=None):
         self.model = DiffusionWrapper(unet, conditioning_key)
         self.first_stage_model, self.scale_factor = first_stage_model, scale_factor
         self.parameterization = parameterization
         self.device = torch.device(device) if device is not None else torch.device(
             "cuda", torch.cuda.current_device()) if torch.cuda.is_available() else torch.device("cpu")
-        self.cond_stage_model = None
+        self.cond_stage_model = cond_stage_model
         self.register_schedule(beta_schedule, timesteps, linear_start, linear_end)
 
     # ddpm.py:118-146 (the buffers the samplers read; fp32 like the reference)
@@ -72,7 +74,15 @@ class LatentDiffusionShim:
         return out[0] if isinstance(out, tuple) and not return_ids else out
 
     def get_learned_conditioning(self, c):
-        raise NotImplementedError("the text encoder (cond stage) is outside the hot path: pass pre-computed embeddings")
+        """ddpm.py:555-566 (cond_stage_forward None): cond_stage_model.encode(c) when it is callable, else
+        cond_stage_model(c)."""
+        m = self.cond_stage_model
+        if m is None:
+            raise NotImplementedError("no cond stage attached: pass cond_stage_model=qdiff_b200.text_encoder."
+                                      "build_text_encoder(...) or pre-computed embeddings")
+        if callable(getattr(m, "encode", None)):
+            return m.encode(c)
+        return m(c)
 
     def decode_first_stage(self, z, predict_cids=False, force_not_quantize=False):
         """ddpm.py:710-767, plain branch (no patch splitting): z / scale_factor -> first_stage_model.decode, on the engine."""

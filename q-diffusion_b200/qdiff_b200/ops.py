@@ -8,7 +8,7 @@ import ctypes as C
 import torch
 
 from . import _lib
-from ._lib import (AttentionDesc, AttentionFpDesc, GemmDesc, GroupNormDesc, Im2colDesc, LayerNormDesc, MiscDesc, QParams,
+from ._lib import (AttentionDesc, AttentionFpDesc, EmbedDesc, GemmDesc, GroupNormDesc, Im2colDesc, LayerNormDesc, MiscDesc, QParams,
                    QuantizeDesc, SamplerDesc, SplitDesc, check, lib, ptr, stream_ptr)
 
 
@@ -201,6 +201,19 @@ def split_bf16x3(desc):
 
 def attention_fp32(desc):
     check(lib().qd_attention_fp32(C.byref(desc), stream_ptr()), "qd_attention_fp32")
+
+
+def embed_desc(ids, tok, pos, out, *, B, T, ld_out=None):
+    """out[b*T + t] = tok[ids[b, t]] + pos[t] (qd_embed_tokens): ids int32 [B*T], tok [vocab, C], pos [>= T, C] fp32."""
+    d = EmbedDesc()
+    d.ids, d.tok, d.pos, d.out = ptr(ids), ptr(tok), ptr(pos), ptr(out)
+    d.B, d.T, d.C, d.vocab = int(B), int(T), int(tok.shape[1]), int(tok.shape[0])
+    d.ld_out = int(ld_out if ld_out is not None else tok.shape[1])
+    return d
+
+
+def embed_tokens(desc):
+    check(lib().qd_embed_tokens(C.byref(desc), stream_ptr()), "qd_embed_tokens")
 
 
 def attention(desc):
