@@ -131,6 +131,9 @@ int qd_qgemm_i8(const qd_gemm_desc* d, qd_stream_t stream);
  *   split > 0: columns [0,split) use q0, columns [split,C) use q1 (split-shortcut,
  *        qdiff/quant_layer.py:257-261)
  *   upsample2x: src is [B,H,W,C], dst [B,2H,2W,C] nearest (F.interpolate, openaimodel.py:116)
+ * Codes: +-inf and values whose quotient x / delta overflows take the rail of their sign; NaN takes qmin.
+ * Vector kernel when C, ld_src, ld_dst and split are multiples of 4, src is 16-byte and dst 4-byte aligned; otherwise a
+ * scalar kernel with the same results.  upsample2x needs the vector kernel: refused (QD_ERR_UNSUPPORTED) otherwise.
  * ------------------------------------------------------------------------------------------ */
 typedef struct qd_quantize_desc {
   const float* src;
@@ -151,7 +154,9 @@ int qd_quantize(const qd_quantize_desc* d, qd_stream_t stream);
  * ddim diffusion.py:32-33 eps 1e-6) [+ scale-shift] [+ SiLU] + up to 3 consumer quantizers.
  * x: fp32 NHWC [B, HW, C] (row pitch ld_x).  ws: 8-byte aligned workspace of at least
  * qd_groupnorm_workspace_floats(B, HW, C, groups) floats (small feature maps take a single-kernel path that
- * does not touch it).
+ * does not touch it).  Alignment (else QD_ERR_UNSUPPORTED): the single-kernel path moves channel pairs, so x and out_f
+ * need 8-byte alignment and ld_f, ld_q even, out_q / raw_q 2-byte alignment; the other paths move channel quads, so x and
+ * out_f need 16-byte alignment, ld_f and ld_q multiples of 4, out_q / raw_q 4-byte alignment.  stats_in: 8-byte aligned.
  * ------------------------------------------------------------------------------------------ */
 typedef struct qd_groupnorm_desc {
   const float* x;
@@ -192,6 +197,10 @@ int qd_groupnorm_quant(const qd_groupnorm_desc* d, qd_stream_t stream);
  * Weight-only mode (quant_act False): activations stay fp32.
  * qd_split_bf16x3 -- dst[m][p][c] = plane p of f(src[m][c]) as bfloat16 (p = 0 hi, 1 mid, 2 lo), c < C; columns C..Cp-1 of
  *   every plane must be zero (allocate dst zeroed).  f: act 0 none, 1 SiLU; upsample2x as in qd_quantize.  ld_dst = 3*Cp.
+ *   Vector kernel when C and ld_src are multiples of 4, src is 16-byte and dst 8-byte aligned; otherwise a scalar kernel
+ *   with the same results.  upsample2x needs the vector kernel: refused (QD_ERR_UNSUPPORTED) otherwise.
+ *   fp32 attention: d + Tk > 12288 is refused (QD_ERR_UNSUPPORTED) unless the 8-row kernel takes the call (not causal,
+ *   Tq >= 256, d, ld_q, ld_k, offsets and head strides multiples of 4, q and k 16-byte aligned).
  * qd_attention_fp32 -- softmax(scale * q k^T) v per (batch, head) in fp32: QuantAttnBlock.forward with use_act_quant
  *   False (qdiff/quant_block.py:360-386) and QKVAttentionLegacy (openaimodel.py:384-406; scale = 1/sqrt(ch) applied to
  *   the product).  q: [B*Tq, ld_q], head h at columns q_off + h*head_stride_q (k, v likewise); out [B*Tq, ld_out].
@@ -269,6 +278,8 @@ typedef struct qd_layernorm_desc {
   float* out_f;          /* optional fp32 output (weight-only state: the consumers take fp32); n_out may then be 0 */
   long long ld_f;
 } qd_layernorm_desc;
+/* Refused (QD_ERR_UNSUPPORTED): C > 2048 or C % 4; x, gamma, beta, out_f not 16-byte aligned; ld_x, ld_f, ld_q not
+ * multiples of 4; out_q not 4-byte aligned. */
 
 int qd_layernorm_quant(const qd_layernorm_desc* d, qd_stream_t stream);
 
@@ -341,6 +352,8 @@ int qd_qattention(const qd_attention_desc* d, qd_stream_t stream);
  *  qd_copy2d: strided fp32 copy (torch.cat along channels, openaimodel.py:776).
  *  qd_nchw_to_nhwc / qd_nhwc_to_nchw: UNet boundary layout change (latents are NCHW fp32).
  *  qd_avgpool2x / qd_upsample2x_f32: Downsample(use_conv=False) / Upsample for resblock_updown.
+ *  copy2d, avgpool and upsample move float4: C (and ld) multiples of 4 and 16-byte aligned src / dst, else
+ *  QD_ERR_UNSUPPORTED.
  * ------------------------------------------------------------------------------------------ */
 int qd_timestep_embedding(const float* t, const float* freqs, int32_t B, int32_t dim, int32_t mode, float* out,
                           qd_stream_t s);
@@ -351,7 +364,9 @@ int qd_avgpool2x(const float* src, float* dst, int32_t B, int32_t H, int32_t W, 
 int qd_upsample2x_f32(const float* src, float* dst, int32_t B, int32_t H, int32_t W, int32_t C, qd_stream_t s);
 /* qd_vq_lookup: the codebook step of VQModelInterface.decode (ldm/models/autoencoder.py:274-283 -> taming's
  *      VectorQuantizer2.forward): for each of `rows` latent pixels z[r, 0..C) (NHWC fp32, row pitch ld_z) the nearest of
- *      the n_e codebook rows by d = sum(z^2) + sum(e^2) - 2 z.e (fp32, lowest index on ties); out = z + (e - z).  C <= 16. */
+ *      the n_e codebook rows by d = sum(z^2) + sum(e^2) - 2 z.e (fp32, lowest index on ties); out = z + (e - z).  C <= 16.
+ *      torch.argmin's order: a NaN distance wins (the first one), so a NaN latent row comes out NaN in its NaN channels;
+ *      a row whose distances are all +inf takes entry 0. */
 /* qd_softmax_rows: in-place softmax over each row of an fp32 [rows, cols] matrix with row pitch ld (the softmax of the
  *      first-stage AttnBlock, model.py:190-192, between its two tensor-core products). */
 int qd_softmax_rows(float* x, long long ld, int32_t rows, int32_t cols, qd_stream_t s);
@@ -449,7 +464,9 @@ typedef struct qd_misc_desc {
 } qd_misc_desc;
 
 int qd_engine_create(int device, qd_engine** out);
-/* desc points at the matching qd_*_desc (qd_misc_desc for kinds 7..12, 15, 16; qd_embed_desc for QD_OP_EMBED); copied. */
+/* desc points at the matching qd_*_desc (qd_misc_desc for kinds 7..12, 15, 16; qd_embed_desc for QD_OP_EMBED); copied.
+ * Every descriptor is checked here with the same rules its qd_* entry point applies (argument ranges, leading dimensions,
+ * alignment of the base pointers), so a descriptor the kernels cannot take is refused when it is added, not at replay. */
 int qd_engine_add_op(qd_engine* e, int kind, const void* desc);
 int qd_engine_num_ops(const qd_engine* e);
 int qd_engine_finalize(qd_engine* e);

@@ -104,7 +104,92 @@ def int_conv3x3(a_codes_nchw, zx, ws4, scale, bias=None):
 
 # ----------------------------------------------------------------------------- elementwise
 def silu(x):
+    """nn.SiLU / nonlinearity (ldm openaimodel.py ResBlock in_layers, ddim diffusion.py:27-29): x * sigmoid(x)."""
     return x * torch.sigmoid(x)
+
+
+def gelu_erf(x):
+    """F.gelu with its default exact-erf form (ldm/modules/attention.py:44): x / 2 * (1 + erf(x / sqrt(2)))."""
+    return 0.5 * x * (1.0 + torch.erf(x / math.sqrt(2.0)))
+
+
+QUICK_GELU_C = float(torch.tensor(1.702, dtype=torch.float32))     # the constant as an fp32 torch op sees it
+
+
+def quick_gelu(x):
+    """transformers' QuickGELUActivation (CLIPMLP, hidden_act "quick_gelu"): x * sigmoid(1.702 x)."""
+    return x * torch.sigmoid(QUICK_GELU_C * x)
+
+
+# ----------------------------------------------------------------------------- normalisation (float64, two-pass)
+def group_norm(x, groups, gamma, beta, eps, ss_scale=None, ss_shift=None, silu_after=False):
+    """GroupNorm32 (ldm util.py:214-216, nn.GroupNorm: biased variance) over NHWC x [B, HW, C] in x's dtype, two-pass
+    mean and variance; with use_scale_shift_norm the ResBlock then applies h * (1 + scale) + shift per image and channel
+    before the SiLU of out_layers (openaimodel.py ResBlock._forward).  Returns (y, mean [B, groups], rstd [B, groups])."""
+    B, HW, C = x.shape
+    xg = x.reshape(B, HW, groups, C // groups)
+    mean = xg.mean(dim=(1, 3))
+    var = ((xg - mean[:, None, :, None]) ** 2).mean(dim=(1, 3))
+    rstd = 1.0 / torch.sqrt(var + eps)
+    y = ((xg - mean[:, None, :, None]) * rstd[:, None, :, None]).reshape(B, HW, C) * gamma + beta
+    if ss_scale is not None:
+        y = y * (1.0 + ss_scale[:, None, :]) + ss_shift[:, None, :]
+    if silu_after:
+        y = silu(y)
+    return y, mean, rstd
+
+
+def layer_norm(x, gamma, beta, eps):
+    """nn.LayerNorm over the last dimension (ldm attention.py BasicTransformerBlock norm1-3, CLIP's layer norms), two-pass."""
+    mean = x.mean(dim=-1, keepdim=True)
+    var = ((x - mean) ** 2).mean(dim=-1, keepdim=True)
+    return (x - mean) / torch.sqrt(var + eps) * gamma + beta
+
+
+# ----------------------------------------------------------------------------- softmax / fp32 attention
+def softmax_rows(x):
+    """softmax over the last dimension (first-stage AttnBlock, model.py:190-192)."""
+    return torch.softmax(x, dim=-1)
+
+
+def attention_fp(q, k, v, scale, causal=False):
+    """softmax(scale q k^T) v per batch-head, q [BH, Tq, d], k / v [BH, Tk, d] (QuantAttnBlock with use_act_quant False,
+    quant_block.py:360-386; QKVAttentionLegacy, openaimodel.py:384-406).  causal: query r attends to keys 0..r only (the
+    CLIP text transformer's causal mask)."""
+    s = torch.einsum('bid,bjd->bij', q, k) * scale
+    if causal:
+        Tq, Tk = s.shape[1], s.shape[2]
+        mask = torch.ones(Tq, Tk, dtype=torch.bool).triu(1)
+        s = s.masked_fill(mask, float("-inf"))
+    return torch.einsum('bij,bjd->bid', torch.softmax(s, dim=-1), v)
+
+
+# ----------------------------------------------------------------------------- VQ first stage
+def _fma32(a, b, c):
+    """fp32 fused multiply-add: the product of two fp32 values is exact in float64, so one float64 add and one rounding
+    to fp32 reproduce fmaf except when the float64 sum itself rounds onto an fp32 tie (double rounding)."""
+    return (a.double() * b.double() + c.double()).float()
+
+
+def vq_nearest(z, cb):
+    """Nearest codebook entry of VectorQuantizer2.forward (taming, legacy branch; the `quantize` step of
+    VQModelInterface.decode, ldm/models/autoencoder.py:274-283), z [rows, C], cb [n_e, C] fp32.  Distances
+    d_j = sum(z^2) + sum(e_j^2) - 2 z.e_j in fp32 with the association the engine uses (each sum of squares left to right,
+    the dot product as a chain of FMAs), then torch.argmin's order: the first NaN, else the lowest index among equal
+    minima.  Returns (index [rows], distances [rows, n_e], out = z + (e - z) in fp32, the straight-through form)."""
+    z = z.float()
+    cb = cb.float()
+    zz = torch.zeros(z.shape[0])
+    ee = torch.zeros(cb.shape[0])
+    dot = torch.zeros(z.shape[0], cb.shape[0])
+    for c in range(z.shape[1]):
+        zz = zz + z[:, c] * z[:, c]
+        ee = ee + cb[:, c] * cb[:, c]
+        dot = _fma32(z[:, c:c + 1], cb[None, :, c], dot)
+    d = (zz[:, None] + ee[None, :]) - 2.0 * dot
+    idx = torch.argmin(torch.where(torch.isnan(d), torch.full_like(d, float("-inf")), d), dim=1)
+    e = cb[idx]
+    return idx, d, z + (e - z)
 
 
 def geglu(x2):

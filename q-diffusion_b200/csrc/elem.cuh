@@ -19,6 +19,8 @@ __device__ __forceinline__ float gelu_erf_f(float x) { return 0.5f * x * (1.0f +
 // quick_gelu of transformers' activations.py (x * sigmoid(1.702 x)), the CLIP text encoder's MLP activation; expf, not
 // __expf: the weight-only planes carry the value to 2^-24
 __device__ __forceinline__ float quick_gelu_f(float x) { return x * (1.0f / (1.0f + expf(-1.702f * x))); }
+// SiLU of the weight-only planes (temb / emb_layers): expf (2 ulp), not __expf, whose error grows as 2 + 1.17 |x| ulp
+__device__ __forceinline__ float silu_accurate_f(float x) { return x / (1.0f + expf(-x)); }
 
 // ------------------------------------------------------------------------------------ quantize
 // One thread = 4 consecutive channels of one row.
@@ -111,7 +113,7 @@ __global__ void split_bf16x3_kernel(const qd_split_desc p) {
 #pragma unroll
     for (int j = 0; j < 4; ++j) {
       float x = v[j];
-      if (p.act == 1) x = x / (1.0f + __expf(-x));          // SiLU with the accurate exponential (this path is fp32-faithful)
+      if (p.act == 1) x = silu_accurate_f(x);
       else if (p.act == 3) x = quick_gelu_f(x);
       const float h = bf16_rn(x);
       const float r1 = x - h;
@@ -135,7 +137,7 @@ __global__ void split_bf16x3_scalar_kernel(const qd_split_desc p) {
     const long long r = i / p.C;
     const int c = (int)(i - r * p.C);
     float x = p.src[r * p.ld_src + c];
-    if (p.act == 1) x = x / (1.0f + __expf(-x));
+    if (p.act == 1) x = silu_accurate_f(x);
     else if (p.act == 2) x *= gelu_erf_f(p.src[r * p.ld_src + p.C + c]);
     else if (p.act == 3) x = quick_gelu_f(x);
     const float h = bf16_rn(x);
@@ -854,6 +856,16 @@ __global__ void __launch_bounds__(256) softmax_rows_kernel(float* __restrict__ x
 // reference's association, argmin with the lowest index on ties, output z + (e - z) (the straight-through form: it
 // rounds).  One warp per pixel, lanes stride over the codebook.
 constexpr int VQ_MAX_C = 16;
+constexpr int VQ_NONE = 0x7fffffff;       // a lane that saw no codebook entry (n_e < 32)
+// torch.argmin's order: a NaN distance is smaller than every number (the first NaN wins), then the lowest index on ties.
+// Every real entry beats VQ_NONE, so the index stays in range even when every distance is +inf or NaN.
+__device__ __forceinline__ bool vq_better(float d, int i, float best, int bi) {
+  if (i == VQ_NONE) return false;
+  if (bi == VQ_NONE) return true;
+  const bool dn = d != d, bn = best != best;
+  if (dn || bn) return dn && (!bn || i < bi);
+  return d < best || (d == best && i < bi);
+}
 __global__ void __launch_bounds__(256) vq_lookup_kernel(const float* __restrict__ z, long long ld_z, const float* __restrict__ cb,
                                                         float* __restrict__ out, long long ld_out, int rows, int C, int n_e) {
   const int lane = threadIdx.x & 31;
@@ -868,7 +880,7 @@ __global__ void __launch_bounds__(256) vq_lookup_kernel(const float* __restrict_
       if (c < C) zz = __fadd_rn(zz, __fmul_rn(zv[c], zv[c]));
     }
     float best = INFINITY;
-    int bi = 0x7fffffff;
+    int bi = VQ_NONE;
     for (int j = lane; j < n_e; j += 32) {
       const float* e = cb + (long long)j * C;
       float ee = 0.f, dot = 0.f;
@@ -881,13 +893,13 @@ __global__ void __launch_bounds__(256) vq_lookup_kernel(const float* __restrict_
         }
       }
       const float dj = __fsub_rn(__fadd_rn(zz, ee), __fmul_rn(2.0f, dot));
-      if (dj < best) { best = dj; bi = j; }
+      if (vq_better(dj, j, best, bi)) { best = dj; bi = j; }
     }
 #pragma unroll
     for (int off = 16; off > 0; off >>= 1) {
       const float ob = __shfl_xor_sync(0xffffffffu, best, off);
       const int oi = __shfl_xor_sync(0xffffffffu, bi, off);
-      if (ob < best || (ob == best && oi < bi)) { best = ob; bi = oi; }
+      if (vq_better(ob, oi, best, bi)) { best = ob; bi = oi; }
     }
     if (lane < C) {
       const float zc = z[r * ld_z + lane];

@@ -471,13 +471,30 @@ int launch_gemm(const GemmPlan& pl, cudaStream_t s) {
 }
 
 // ------------------------------------------------------------------ elementwise launchers
-int launch_quantize(const qd_quantize_desc& d, cudaStream_t s) {
+// Each launcher's descriptor checks live in a validate_* function that qd_engine_add_op runs too, so that a descriptor the
+// kernels cannot take is refused when it is added to a program rather than surfacing mid-graph as a misaligned access.
+// Vector paths need their base pointers and leading dimensions aligned to the access width; where a scalar kernel exists
+// (quantize, split, im2col) a misaligned descriptor runs that one instead.
+bool aligned(const void* p, int bytes) { return ((uintptr_t)p & (uintptr_t)(bytes - 1)) == 0; }
+
+bool quantize_vec(const qd_quantize_desc& d) {
+  return (d.C % 4 == 0) && (d.ld_src % 4 == 0) && (d.ld_dst % 4 == 0) && (d.split % 4 == 0) && aligned(d.src, 16) &&
+         aligned(d.dst, 4);
+}
+
+int validate_quantize(const qd_quantize_desc& d) {
   if (!d.src || !d.dst || d.M <= 0 || d.C <= 0) return fail(QD_ERR_BAD_ARG, "quantize: bad args");
   if (d.q0.qmax - d.q0.qmin > 255 || d.q1.qmax - d.q1.qmin > 255)
     return fail(QD_ERR_UNSUPPORTED, "quantize: the engine emits 8-bit codes; quantizer range [%d, %d] is wider", d.q0.qmin, d.q0.qmax);
-  const bool vec = (d.C % 4 == 0) && (d.ld_src % 4 == 0) && (d.ld_dst % 4 == 0) && (d.split % 4 == 0);
-  if (d.upsample2x && !vec) return fail(QD_ERR_UNSUPPORTED, "quantize: upsample needs C %% 4 == 0");
-  if (vec) {
+  if (!aligned(d.src, 4)) return fail(QD_ERR_UNSUPPORTED, "quantize: src must be 4-byte aligned");
+  if (d.upsample2x && !quantize_vec(d))
+    return fail(QD_ERR_UNSUPPORTED, "quantize: upsample needs C, ld_src, ld_dst, split %% 4 == 0, src 16-byte and dst 4-byte aligned");
+  return QD_OK;
+}
+
+int launch_quantize(const qd_quantize_desc& d, cudaStream_t s) {
+  if (int rc = validate_quantize(d)) return rc;
+  if (quantize_vec(d)) {
     const long long rows = d.upsample2x ? (long long)d.B * 4 * d.H * d.W : d.M;
     launch_k(qd::quantize_kernel, grid_for(rows * (d.C / 4), 256), 256, 0, s, d);
   } else {
@@ -508,41 +525,75 @@ int use_stats_env() {
   return v;
 }
 
-int launch_groupnorm(const qd_groupnorm_desc& d, cudaStream_t s) {
-  if (!d.x || !d.gamma || !d.beta) return fail(QD_ERR_BAD_ARG, "groupnorm: null arg");
-  if (d.groups <= 0 || d.groups > qd::GN_MAX_GROUPS || d.C % 4 || d.C % d.groups || d.ld_x % 4)
-    return fail(QD_ERR_UNSUPPORTED, "groupnorm: C=%d groups=%d", d.C, d.groups);
-  if (d.n_out < 0 || d.n_out > 3) return fail(QD_ERR_BAD_ARG, "groupnorm: n_out");
-  if (d.raw_q && ((d.raw_split & 3) || (d.ld_raw & 3) || d.raw_split < 0))
-    return fail(QD_ERR_BAD_ARG, "groupnorm: raw output needs raw_split %% 4 == 0 and ld_raw %% 4 == 0");
+enum GnPath { GN_FUSED, GN_FROM_STATS, GN_PARTIAL };
+
+// Which of the three GroupNorm paths launch_groupnorm takes for a descriptor (the checks of validate_groupnorm passed).
+GnPath gn_path(const qd_groupnorm_desc& d) {
   const int cpg = d.C / d.groups;
   // ---- single-kernel path: the (image, group) slab fits the registers of one block
-  {
-    bool ok = (cpg % 2 == 0) && cpg <= 128 && (d.ld_x % 2 == 0) && (!d.out_f || d.ld_f % 2 == 0);
-    for (int o = 0; o < d.n_out; ++o) ok = ok && (d.ld_q[o] % 2 == 0);
-    const long long units = (long long)d.HW * (cpg / 2);
-    static const int force = [] {   // QDIFF_GN=fused|split: A/B switch for profiling
-      const char* e = getenv("QDIFF_GN");
-      return !e ? 0 : (!strcmp(e, "fused") ? 1 : (!strcmp(e, "split") ? 2 : 0));
-    }();
-    const long long limit = force == 1 ? 512LL * qd::GN_NU : (force == 2 ? 0 : 256LL * qd::GN_NU);
-    // The one-block-per-(image, group) kernel reads cpg * 4 bytes per pixel out of every C * 4 (sector-inefficient for
-    // narrow groups) and launches B * groups blocks: it only pays in the launch-latency regime.  The three-kernel path
-    // (statistics from the producing GEMMs' slab sums, then a coalesced apply pass) takes everything else: maps above ~2 M
-    // elements or with more than 2048 blocks, and above ~0.5 M elements when the producing GEMMs left slab statistics.
-    // (Thresholds from per-op timings on the previous GPU generation; not re-measured on the H100.)
-    const long long elems = (long long)d.B * d.HW * d.C;
-    const bool small_problem = elems <= ((d.stats_in && use_stats_env()) ? (512LL << 10) : (2LL << 20)) && (long long)d.B * d.groups <= 2048;
-    if (ok && units <= limit && (force == 1 || small_problem)) {
-      int threads = units <= 256LL * qd::GN_NU ? 256 : 512;
-      if (units < 256) threads = (int)((units + 31) / 32 * 32);
-      if (threads < cpg / 2) threads = (cpg / 2 + 31) / 32 * 32;
-      launch_k(qd::gn_fused_small_kernel, dim3(d.groups, d.B), threads, 0, s, d);
-      return check_launch("gn_fused_small_kernel");
-    }
+  bool ok = (cpg % 2 == 0) && cpg <= 128 && (d.ld_x % 2 == 0) && (!d.out_f || d.ld_f % 2 == 0);
+  for (int o = 0; o < d.n_out; ++o) ok = ok && (d.ld_q[o] % 2 == 0);
+  const long long units = (long long)d.HW * (cpg / 2);
+  static const int force = [] {   // QDIFF_GN=fused|split: A/B switch for profiling
+    const char* e = getenv("QDIFF_GN");
+    return !e ? 0 : (!strcmp(e, "fused") ? 1 : (!strcmp(e, "split") ? 2 : 0));
+  }();
+  const long long limit = force == 1 ? 512LL * qd::GN_NU : (force == 2 ? 0 : 256LL * qd::GN_NU);
+  // The one-block-per-(image, group) kernel reads cpg * 4 bytes per pixel out of every C * 4 (sector-inefficient for
+  // narrow groups) and launches B * groups blocks: it only pays in the launch-latency regime.  The three-kernel path
+  // (statistics from the producing GEMMs' slab sums, then a coalesced apply pass) takes everything else: maps above ~2 M
+  // elements or with more than 2048 blocks, and above ~0.5 M elements when the producing GEMMs left slab statistics.
+  // (Thresholds from per-op timings on the previous GPU generation; not re-measured on the H100.)
+  const long long elems = (long long)d.B * d.HW * d.C;
+  const bool small_problem = elems <= ((d.stats_in && use_stats_env()) ? (512LL << 10) : (2LL << 20)) && (long long)d.B * d.groups <= 2048;
+  if (ok && units <= limit && (force == 1 || small_problem)) return GN_FUSED;
+  return (d.stats_in && use_stats_env()) ? GN_FROM_STATS : GN_PARTIAL;
+}
+
+int validate_groupnorm(const qd_groupnorm_desc& d) {
+  if (!d.x || !d.gamma || !d.beta || d.B <= 0 || d.HW <= 0) return fail(QD_ERR_BAD_ARG, "groupnorm: null arg or empty map");
+  if (d.groups <= 0 || d.groups > qd::GN_MAX_GROUPS || d.C <= 0 || d.C % 4 || d.C % d.groups || d.ld_x % 4)
+    return fail(QD_ERR_UNSUPPORTED, "groupnorm: C=%d groups=%d", d.C, d.groups);
+  if (d.n_out < 0 || d.n_out > 3) return fail(QD_ERR_BAD_ARG, "groupnorm: n_out");
+  for (int o = 0; o < d.n_out; ++o)
+    if (!d.out_q[o]) return fail(QD_ERR_BAD_ARG, "groupnorm: out_q[%d] is NULL", o);
+  if (d.ss_scale && !d.ss_shift) return fail(QD_ERR_BAD_ARG, "groupnorm: scale-shift needs both operands");
+  if (d.raw_q && ((d.raw_split & 3) || (d.ld_raw & 3) || d.raw_split < 0))
+    return fail(QD_ERR_BAD_ARG, "groupnorm: raw output needs raw_split %% 4 == 0 and ld_raw %% 4 == 0");
+  // the fused kernel moves channel pairs (float2 loads and stores, 16-bit code pairs); the apply kernel channel quads
+  // (float4, 32-bit code quads)
+  const GnPath path = gn_path(d);
+  const int w = path == GN_FUSED ? 2 : 4;
+  if (!aligned(d.x, 4 * w)) return fail(QD_ERR_UNSUPPORTED, "groupnorm: x must be %d-byte aligned", 4 * w);
+  if (d.out_f && (!aligned(d.out_f, 4 * w) || d.ld_f % w))
+    return fail(QD_ERR_UNSUPPORTED, "groupnorm: out_f needs %d-byte alignment and ld_f %% %d == 0", 4 * w, w);
+  for (int o = 0; o < d.n_out; ++o)
+    if (!aligned(d.out_q[o], w) || d.ld_q[o] % w)
+      return fail(QD_ERR_UNSUPPORTED, "groupnorm: out_q[%d] needs %d-byte alignment and ld_q %% %d == 0", o, w, w);
+  if (d.raw_q && !aligned(d.raw_q, w)) return fail(QD_ERR_UNSUPPORTED, "groupnorm: raw_q must be %d-byte aligned", w);
+  if (path != GN_FUSED) {
+    if (!d.ws) return fail(QD_ERR_BAD_ARG, "groupnorm: workspace required");
+    if (!aligned(d.ws, 8)) return fail(QD_ERR_BAD_ARG, "groupnorm: workspace must be 8-byte aligned");
   }
-  if (!d.ws) return fail(QD_ERR_BAD_ARG, "groupnorm: workspace required");
-  if ((uintptr_t)d.ws & 7) return fail(QD_ERR_BAD_ARG, "groupnorm: workspace must be 8-byte aligned");
+  if (path == GN_FROM_STATS) {
+    if (d.HW % 32) return fail(QD_ERR_BAD_ARG, "groupnorm: stats_in needs HW %% 32 == 0");
+    if (!aligned(d.stats_in, 8)) return fail(QD_ERR_UNSUPPORTED, "groupnorm: stats_in must be 8-byte aligned");
+  }
+  return QD_OK;
+}
+
+int launch_groupnorm(const qd_groupnorm_desc& d, cudaStream_t s) {
+  if (int rc = validate_groupnorm(d)) return rc;
+  const int cpg = d.C / d.groups;
+  const GnPath path = gn_path(d);
+  if (path == GN_FUSED) {
+    const long long units = (long long)d.HW * (cpg / 2);
+    int threads = units <= 256LL * qd::GN_NU ? 256 : 512;
+    if (units < 256) threads = (int)((units + 31) / 32 * 32);
+    if (threads < cpg / 2) threads = (cpg / 2 + 31) / 32 * 32;
+    launch_k(qd::gn_fused_small_kernel, dim3(d.groups, d.B), threads, 0, s, d);
+    return check_launch("gn_fused_small_kernel");
+  }
   const int slab = gn_slab_rows(d.B, d.HW);
   const int nslab = (d.HW + slab - 1) / slab;
   double* part = reinterpret_cast<double*>(d.ws);
@@ -552,10 +603,8 @@ int launch_groupnorm(const qd_groupnorm_desc& d, cudaStream_t s) {
   if (threads > 256) threads = 256;
   if (threads < 2 * d.groups) threads = (2 * d.groups + 31) / 32 * 32;
   int rc;
-  const int use_stats = use_stats_env();
-  if (d.stats_in && use_stats) {
+  if (path == GN_FROM_STATS) {
     // the producing GEMMs left per-slab column sums: no pass over x for the statistics
-    if (d.HW % 32) return fail(QD_ERR_BAD_ARG, "groupnorm: stats_in needs HW %% 32 == 0");
     launch_k(qd::gn_finalize_from_stats_kernel, dim3(d.groups, d.B), 128, 0, s, reinterpret_cast<const float2*>(d.stats_in),
                                                                          d.ld_stats_in, d.HW, d.C, d.groups, d.eps, stats);
     rc = check_launch("gn_finalize_from_stats_kernel");
@@ -602,11 +651,23 @@ int launch_layernorm_t(const qd_layernorm_desc& d, cudaStream_t s) {
   return check_launch("layernorm_quant_kernel");
 }
 
-int launch_layernorm(const qd_layernorm_desc& d, cudaStream_t s) {
-  if (!d.x || !d.gamma || !d.beta) return fail(QD_ERR_BAD_ARG, "layernorm: null arg");
-  if (d.C % 4 || d.ld_x % 4) return fail(QD_ERR_UNSUPPORTED, "layernorm: C=%d", d.C);
+int validate_layernorm(const qd_layernorm_desc& d) {
+  if (!d.x || !d.gamma || !d.beta || d.M <= 0) return fail(QD_ERR_BAD_ARG, "layernorm: null arg or M <= 0");
+  if (d.C <= 0 || d.C % 4 || d.ld_x % 4) return fail(QD_ERR_UNSUPPORTED, "layernorm: C=%d", d.C);
+  if (d.C > 2048) return fail(QD_ERR_UNSUPPORTED, "layernorm: C=%d exceeds 2048", d.C);
   if (d.n_out < 0 || d.n_out > 3 || (d.n_out == 0 && !d.out_f)) return fail(QD_ERR_BAD_ARG, "layernorm: n_out");
   if (d.out_f && (d.ld_f & 3)) return fail(QD_ERR_UNSUPPORTED, "layernorm: ld_f");
+  // float4 loads of x, gamma, beta; float4 stores of out_f; 32-bit stores of four codes
+  if (!aligned(d.x, 16) || !aligned(d.gamma, 16) || !aligned(d.beta, 16) || (d.out_f && !aligned(d.out_f, 16)))
+    return fail(QD_ERR_UNSUPPORTED, "layernorm: x, gamma, beta and out_f must be 16-byte aligned");
+  for (int o = 0; o < d.n_out; ++o)
+    if (!d.out_q[o] || !aligned(d.out_q[o], 4) || (d.ld_q[o] & 3))
+      return fail(QD_ERR_UNSUPPORTED, "layernorm: out_q[%d] needs 4-byte alignment and ld_q %% 4 == 0", o);
+  return QD_OK;
+}
+
+int launch_layernorm(const qd_layernorm_desc& d, cudaStream_t s) {
+  if (int rc = validate_layernorm(d)) return rc;
   const int nvec = (d.C / 4 + 31) / 32;
   switch (nvec) {
     case 1: return launch_layernorm_t<1>(d, s);
@@ -621,12 +682,25 @@ int launch_layernorm(const qd_layernorm_desc& d, cudaStream_t s) {
   }
 }
 
-int launch_split3(const qd_split_desc& d, cudaStream_t s) {
+// the vector kernel loads float4 and stores four bfloat16 per plane as one 8-byte word
+bool split_vec(const qd_split_desc& d) {
+  return !(d.C & 3) && !(d.ld_src & 3) && aligned(d.src, 16) && aligned(d.dst, 8);
+}
+
+int validate_split3(const qd_split_desc& d) {
   if (!d.src || !d.dst || d.M <= 0 || d.C <= 0) return fail(QD_ERR_BAD_ARG, "split: bad args");
+  if (d.act < 0 || d.act > 3) return fail(QD_ERR_BAD_ARG, "split: act %d", d.act);
   if ((d.Cp & 3) || d.Cp < d.C || d.ld_dst < 3LL * d.Cp || (d.ld_dst & 3))
     return fail(QD_ERR_UNSUPPORTED, "split: Cp=%d must be a multiple of 4, >= C, with ld_dst >= 3*Cp", d.Cp);
-  if ((d.C & 3) || (d.ld_src & 3)) {
-    if (d.upsample2x) return fail(QD_ERR_UNSUPPORTED, "split: upsample needs C %% 4 == 0");
+  if (!aligned(d.src, 4) || !aligned(d.dst, 2)) return fail(QD_ERR_UNSUPPORTED, "split: src / dst misaligned for their types");
+  if (d.upsample2x && !split_vec(d))
+    return fail(QD_ERR_UNSUPPORTED, "split: upsample needs C, ld_src %% 4 == 0, src 16-byte and dst 8-byte aligned");
+  return QD_OK;
+}
+
+int launch_split3(const qd_split_desc& d, cudaStream_t s) {
+  if (int rc = validate_split3(d)) return rc;
+  if (!split_vec(d)) {
     launch_k(qd::split_bf16x3_scalar_kernel, grid_for((long long)d.M * d.C, 256), 256, 0, s, d);
     return check_launch("split_bf16x3_scalar_kernel");
   }
@@ -635,38 +709,76 @@ int launch_split3(const qd_split_desc& d, cudaStream_t s) {
   return check_launch("split_bf16x3_kernel");
 }
 
-int launch_attention_fp(const qd_attention_fp_desc& d, cudaStream_t s) {
+// long sequences (never causal: the text encoder's T = 77 takes the one-row kernel): AFP_R query rows per block share the
+// K / V rows they read (K/V traffic / AFP_R).  Its phase 1 reads K as float4.
+size_t afp_rows_smem(const qd_attention_fp_desc& d) {
+  return (size_t)qd::AFP_R * (d.d + qd::afp_tk_pitch(d.Tk)) * sizeof(float);
+}
+bool afp_rows(const qd_attention_fp_desc& d) {
+  const bool vec = !(d.d & 3) && !(d.ld_q & 3) && !(d.ld_k & 3) && !(d.q_off & 3) && !(d.k_off & 3) && !(d.head_stride_q & 3) &&
+                   !(d.head_stride_k & 3) && aligned(d.q, 16) && aligned(d.k, 16);
+  return !d.causal && d.Tq >= 256 && afp_rows_smem(d) <= 200 * 1024 && vec;
+}
+
+int validate_attention_fp(const qd_attention_fp_desc& d) {
   if (!d.q || !d.k || !d.v || !d.out || d.B <= 0 || d.heads <= 0 || d.d <= 0 || d.Tq <= 0 || d.Tk <= 0)
     return fail(QD_ERR_BAD_ARG, "attention_fp32: bad args");
   if (d.causal != 0 && d.causal != 1) return fail(QD_ERR_BAD_ARG, "attention_fp32: causal must be 0 or 1 (got %d)", d.causal);
   if (d.causal && d.Tq != d.Tk) return fail(QD_ERR_UNSUPPORTED, "attention_fp32: causal needs Tq == Tk (got %d, %d)", d.Tq, d.Tk);
-  // long sequences (never causal: the text encoder's T = 77 takes the one-row kernel): AFP_R query rows per block share the K / V rows they read (K/V traffic / AFP_R)
-  const size_t smem_rows = (size_t)qd::AFP_R * (d.d + qd::afp_tk_pitch(d.Tk)) * sizeof(float);
-  const bool aligned = !(d.d & 3) && !(d.ld_q & 3) && !(d.ld_k & 3) && !(d.q_off & 3) && !(d.k_off & 3) && !(d.head_stride_q & 3) &&
-                       !(d.head_stride_k & 3) && !((uintptr_t)d.q & 15) && !((uintptr_t)d.k & 15);
-  if (!d.causal && d.Tq >= 256 && smem_rows <= 200 * 1024 && aligned) {
+  if (!aligned(d.q, 4) || !aligned(d.k, 4) || !aligned(d.v, 4) || !aligned(d.out, 4))
+    return fail(QD_ERR_UNSUPPORTED, "attention_fp32: q, k, v and out must be 4-byte aligned");
+  if (!afp_rows(d) && (size_t)(d.d + d.Tk) * sizeof(float) > 48 * 1024)
+    return fail(QD_ERR_UNSUPPORTED, "attention_fp32: d + Tk = %d exceeds 12288 floats of shared memory", d.d + d.Tk);
+  return QD_OK;
+}
+
+int launch_attention_fp(const qd_attention_fp_desc& d, cudaStream_t s) {
+  if (int rc = validate_attention_fp(d)) return rc;
+  if (afp_rows(d)) {
     static std::atomic<unsigned long long> optin{0};
     if (int rc = ensure_smem_optin(qd::attention_fp32_rows_kernel, 200 * 1024, optin, "attention_fp32_rows")) return rc;
-    launch_k(qd::attention_fp32_rows_kernel, dim3((d.Tq + qd::AFP_R - 1) / qd::AFP_R, d.B * d.heads), 256, smem_rows, s, d);
+    launch_k(qd::attention_fp32_rows_kernel, dim3((d.Tq + qd::AFP_R - 1) / qd::AFP_R, d.B * d.heads), 256, afp_rows_smem(d), s, d);
     return check_launch("attention_fp32_rows_kernel");
   }
+  // the dynamic score row may take the whole default 48 KB: the kernel's static reduction slots come on top, which needs
+  // the opt-in (without it d + Tk = 12288 failed to launch)
+  static std::atomic<unsigned long long> optin1{0};
+  if (int rc = ensure_smem_optin(qd::attention_fp32_kernel, 48 * 1024, optin1, "attention_fp32")) return rc;
   const size_t smem = (size_t)(d.d + d.Tk) * sizeof(float);
-  if (smem > 48 * 1024) return fail(QD_ERR_UNSUPPORTED, "attention_fp32: d + Tk = %d exceeds 12288 floats of shared memory", d.d + d.Tk);
   launch_k(qd::attention_fp32_kernel, dim3(d.Tq, d.B * d.heads), 128, smem, s, d);
   return check_launch("attention_fp32_kernel");
 }
 
-int launch_embed(const qd_embed_desc& d, cudaStream_t s) {
+int validate_embed(const qd_embed_desc& d) {
   if (!d.ids || !d.tok || !d.pos || !d.out || d.B <= 0 || d.T <= 0 || d.C <= 0 || d.vocab <= 0 || d.ld_out < d.C)
     return fail(QD_ERR_BAD_ARG, "embed_tokens: bad args (B=%d T=%d C=%d vocab=%d ld_out=%lld)", d.B, d.T, d.C, d.vocab, d.ld_out);
+  if (!aligned(d.ids, 4) || !aligned(d.tok, 4) || !aligned(d.pos, 4) || !aligned(d.out, 4))
+    return fail(QD_ERR_UNSUPPORTED, "embed_tokens: ids, tok, pos and out must be 4-byte aligned");
+  return QD_OK;
+}
+
+int launch_embed(const qd_embed_desc& d, cudaStream_t s) {
+  if (int rc = validate_embed(d)) return rc;
   launch_k(qd::embed_tokens_kernel, grid_for((long long)d.B * d.T * d.C, 256), 256, 0, s, d);
   return check_launch("embed_tokens_kernel");
 }
 
-int launch_im2col(const qd_im2col_desc& d, cudaStream_t s) {
+// 16 channels of one tap per thread: uint4 loads and stores
+bool im2col_vec(const qd_im2col_desc& d) {
+  return (d.C % 16) == 0 && d.ld_dst == 9 * d.C && (d.ld_dst % 16) == 0 && aligned(d.src, 16) && aligned(d.dst, 16);
+}
+
+int validate_im2col(const qd_im2col_desc& d) {
   if (!d.src || !d.dst) return fail(QD_ERR_BAD_ARG, "im2col: null arg");
+  if (d.B <= 0 || d.H <= 0 || d.W <= 0 || d.C <= 0 || d.Ho <= 0 || d.Wo <= 0 || d.stride <= 0)
+    return fail(QD_ERR_BAD_ARG, "im2col: empty geometry");
   if (d.ld_dst < 9 * d.C) return fail(QD_ERR_BAD_ARG, "im2col: ld_dst too small");
-  if ((d.C % 16) == 0 && d.ld_dst == 9 * d.C && (d.ld_dst % 16) == 0) {
+  return QD_OK;
+}
+
+int launch_im2col(const qd_im2col_desc& d, cudaStream_t s) {
+  if (int rc = validate_im2col(d)) return rc;
+  if (im2col_vec(d)) {
     launch_k(qd::im2col_vec_kernel, grid_for((long long)d.B * d.Ho * d.Wo * 9 * (d.C / 16), 256), 256, 0, s, d);
     return check_launch("im2col_vec_kernel");
   }
@@ -809,7 +921,7 @@ int launch_attention_wg(const qd_attention_desc& d, cudaStream_t s) {
   }
 }
 
-int launch_attention(const qd_attention_desc& d, cudaStream_t s) {
+int validate_attention(const qd_attention_desc& d) {
   if (!d.q || !d.k || !d.vt || (!d.out && !d.out_q)) return fail(QD_ERR_BAD_ARG, "attention: null arg");
   if (d.out_q && (d.ld_out_q & 1)) return fail(QD_ERR_UNSUPPORTED, "attention: ld_out_q");
   if (d.q_signed != d.k_signed) return fail(QD_ERR_UNSUPPORTED, "attention: q/k signedness differ");
@@ -825,6 +937,11 @@ int launch_attention(const qd_attention_desc& d, cudaStream_t s) {
   if ((d.q_off | d.head_stride_q | (int)d.ld_q) & 3) return fail(QD_ERR_UNSUPPORTED, "attention: q needs 4-byte alignment");
   if ((d.k_off | d.head_stride_k | (int)d.ld_k | d.d) & 7) return fail(QD_ERR_UNSUPPORTED, "attention: k rows need 8-byte alignment");
   if (d.out && (d.ld_out % 2)) return fail(QD_ERR_UNSUPPORTED, "attention: ld_out");
+  return QD_OK;
+}
+
+int launch_attention(const qd_attention_desc& d, cudaStream_t s) {
+  if (int rc = validate_attention(d)) return rc;
   if (d.qk_f16) {      // fp16 centred-code Q / K (QK^T on f16 x f16 -> f32 MMAs, exact), d <= 64, any Tk
     if (attention_wg_eligible(d)) return launch_attention_wg(d, s);
     switch (d.d) {
@@ -857,14 +974,45 @@ int launch_attention(const qd_attention_desc& d, cudaStream_t s) {
   }
 }
 
-int launch_misc(int kind, const qd_misc_desc& m, cudaStream_t s) {
+int validate_misc(int kind, const qd_misc_desc& m) {
+  if (!m.src || !m.dst) return fail(QD_ERR_BAD_ARG, "misc %d: null src / dst", kind);
+  if (!aligned(m.src, 4) || !aligned(m.dst, 4)) return fail(QD_ERR_UNSUPPORTED, "misc %d: src / dst must be 4-byte aligned", kind);
   switch (kind) {
     case QD_OP_TIMESTEP_EMB:
       if (!m.aux) return fail(QD_ERR_BAD_ARG, "timestep_embedding: missing frequency table");
+      return QD_OK;
+    case QD_OP_COPY2D:      // float4 rows
+      if (m.b % 4 || m.ld_src % 4 || m.ld_dst % 4 || !aligned(m.src, 16) || !aligned(m.dst, 16))
+        return fail(QD_ERR_UNSUPPORTED, "copy2d: C, ld_src, ld_dst %% 4 == 0 and 16-byte aligned src / dst");
+      return QD_OK;
+    case QD_OP_NCHW_TO_NHWC:
+    case QD_OP_NHWC_TO_NCHW:
+      return QD_OK;
+    case QD_OP_AVGPOOL2X:   // float4 channel quads
+    case QD_OP_UPSAMPLE2X:
+      if (m.d % 4 || !aligned(m.src, 16) || !aligned(m.dst, 16))
+        return fail(QD_ERR_UNSUPPORTED, "%s: C %% 4 == 0 and 16-byte aligned src / dst", kind == QD_OP_AVGPOOL2X ? "avgpool" : "upsample");
+      return QD_OK;
+    case QD_OP_SOFTMAX_ROWS:
+      if (m.a <= 0 || m.b <= 0 || m.ld_src < m.b || m.src != m.dst) return fail(QD_ERR_BAD_ARG, "softmax_rows: in place, rows=%d cols=%d", m.a, m.b);
+      return QD_OK;
+    case QD_OP_VQ_LOOKUP:
+      if (!m.aux || m.a <= 0 || m.b <= 0 || m.b > qd::VQ_MAX_C || m.c <= 0 || m.ld_src < m.b || m.ld_dst < m.b)
+        return fail(QD_ERR_BAD_ARG, "vq_lookup: bad args (rows=%d, C=%d <= %d, n_e=%d)", m.a, m.b, qd::VQ_MAX_C, m.c);
+      if (!aligned(m.aux, 4)) return fail(QD_ERR_UNSUPPORTED, "vq_lookup: codebook must be 4-byte aligned");
+      return QD_OK;
+    default:
+      return fail(QD_ERR_BAD_ARG, "misc: unknown kind %d", kind);
+  }
+}
+
+int launch_misc(int kind, const qd_misc_desc& m, cudaStream_t s) {
+  if (int rc = validate_misc(kind, m)) return rc;
+  switch (kind) {
+    case QD_OP_TIMESTEP_EMB:
       launch_k(qd::timestep_embedding_kernel, grid_for((long long)m.a * (m.b / 2), 128), 128, 0, s, m.src, m.aux, m.a, m.b, m.c, m.dst);
       return check_launch("timestep_embedding_kernel");
     case QD_OP_COPY2D:
-      if (m.b % 4 || m.ld_src % 4 || m.ld_dst % 4) return fail(QD_ERR_UNSUPPORTED, "copy2d: alignment");
       launch_k(qd::copy2d_kernel, grid_for((long long)m.a * (m.b / 4), 256), 256, 0, s, m.src, m.ld_src, m.dst, m.ld_dst, m.a, m.b);
       return check_launch("copy2d_kernel");
     case QD_OP_NCHW_TO_NHWC:
@@ -874,20 +1022,15 @@ int launch_misc(int kind, const qd_misc_desc& m, cudaStream_t s) {
       launch_k(qd::nhwc_to_nchw_kernel, grid_for((long long)m.a * m.b * m.c, 256), 256, 0, s, m.src, m.dst, m.a, m.b, m.c);
       return check_launch("nhwc_to_nchw_kernel");
     case QD_OP_AVGPOOL2X:
-      if (m.d % 4) return fail(QD_ERR_UNSUPPORTED, "avgpool: C %% 4");
       launch_k(qd::avgpool2x_kernel, grid_for((long long)m.a * (m.b / 2) * (m.c / 2) * (m.d / 4), 256), 256, 0, s, m.src, m.dst, m.a, m.b, m.c, m.d);
       return check_launch("avgpool2x_kernel");
     case QD_OP_UPSAMPLE2X:
-      if (m.d % 4) return fail(QD_ERR_UNSUPPORTED, "upsample: C %% 4");
       launch_k(qd::upsample2x_f32_kernel, grid_for((long long)m.a * m.b * m.c * m.d, 256), 256, 0, s, m.src, m.dst, m.a, m.b, m.c, m.d);
       return check_launch("upsample2x_f32_kernel");
     case QD_OP_SOFTMAX_ROWS:
-      if (m.a <= 0 || m.b <= 0 || m.ld_src < m.b || m.src != m.dst) return fail(QD_ERR_BAD_ARG, "softmax_rows: in place, rows=%d cols=%d", m.a, m.b);
       launch_k(qd::softmax_rows_kernel, dim3(m.a), 256, 0, s, m.dst, m.ld_src, m.b);
       return check_launch("softmax_rows_kernel");
     case QD_OP_VQ_LOOKUP:
-      if (!m.aux || m.a <= 0 || m.b <= 0 || m.b > qd::VQ_MAX_C || m.c <= 0 || m.ld_src < m.b || m.ld_dst < m.b)
-        return fail(QD_ERR_BAD_ARG, "vq_lookup: bad args (rows=%d, C=%d <= %d, n_e=%d)", m.a, m.b, qd::VQ_MAX_C, m.c);
       launch_k(qd::vq_lookup_kernel, grid_for((long long)m.a * 32, 256), 256, 0, s, m.src, m.ld_src, m.aux, m.dst, m.ld_dst, m.a, m.b, m.c);
       return check_launch("vq_lookup_kernel");
     default:
@@ -1056,26 +1199,29 @@ int qd_engine_add_op(qd_engine* e, int kind, const void* desc) {
   if (!g.ok) return fail(QD_ERR_CUDA, "cudaSetDevice(%d) failed", e->device);
   Op op;
   op.kind = kind;
+  int rc = QD_OK;
   switch (kind) {
-    case QD_OP_GEMM: {
-      int rc = plan_gemm(reinterpret_cast<const qd_gemm_desc*>(desc), &op.gemm);
-      if (rc) return rc;
+    case QD_OP_GEMM: rc = plan_gemm(reinterpret_cast<const qd_gemm_desc*>(desc), &op.gemm); break;
+    // the launchers' own checks, so that a descriptor the kernels cannot take is refused here and not at replay
+    case QD_OP_QUANTIZE: op.quant = *reinterpret_cast<const qd_quantize_desc*>(desc); rc = validate_quantize(op.quant); break;
+    case QD_OP_GROUPNORM: op.gn = *reinterpret_cast<const qd_groupnorm_desc*>(desc); rc = validate_groupnorm(op.gn); break;
+    case QD_OP_LAYERNORM: op.ln = *reinterpret_cast<const qd_layernorm_desc*>(desc); rc = validate_layernorm(op.ln); break;
+    case QD_OP_IM2COL: op.im2col = *reinterpret_cast<const qd_im2col_desc*>(desc); rc = validate_im2col(op.im2col); break;
+    case QD_OP_ATTENTION: op.att = *reinterpret_cast<const qd_attention_desc*>(desc); rc = validate_attention(op.att); break;
+    case QD_OP_SPLIT3: op.split = *reinterpret_cast<const qd_split_desc*>(desc); rc = validate_split3(op.split); break;
+    case QD_OP_ATTENTION_FP:
+      op.attfp = *reinterpret_cast<const qd_attention_fp_desc*>(desc);
+      rc = validate_attention_fp(op.attfp);
       break;
-    }
-    case QD_OP_QUANTIZE: op.quant = *reinterpret_cast<const qd_quantize_desc*>(desc); break;
-    case QD_OP_GROUPNORM: op.gn = *reinterpret_cast<const qd_groupnorm_desc*>(desc); break;
-    case QD_OP_LAYERNORM: op.ln = *reinterpret_cast<const qd_layernorm_desc*>(desc); break;
-    case QD_OP_IM2COL: op.im2col = *reinterpret_cast<const qd_im2col_desc*>(desc); break;
-    case QD_OP_ATTENTION: op.att = *reinterpret_cast<const qd_attention_desc*>(desc); break;
-    case QD_OP_SPLIT3: op.split = *reinterpret_cast<const qd_split_desc*>(desc); break;
-    case QD_OP_ATTENTION_FP: op.attfp = *reinterpret_cast<const qd_attention_fp_desc*>(desc); break;
-    case QD_OP_EMBED: op.embed = *reinterpret_cast<const qd_embed_desc*>(desc); break;
+    case QD_OP_EMBED: op.embed = *reinterpret_cast<const qd_embed_desc*>(desc); rc = validate_embed(op.embed); break;
     case QD_OP_TIMESTEP_EMB: case QD_OP_COPY2D: case QD_OP_NCHW_TO_NHWC: case QD_OP_NHWC_TO_NCHW:
     case QD_OP_AVGPOOL2X: case QD_OP_UPSAMPLE2X: case QD_OP_VQ_LOOKUP: case QD_OP_SOFTMAX_ROWS:
       op.misc = *reinterpret_cast<const qd_misc_desc*>(desc);
+      rc = validate_misc(kind, op.misc);
       break;
     default: return fail(QD_ERR_BAD_ARG, "unknown op kind %d", kind);
   }
+  if (rc) return rc;
   e->ops.push_back(op);
   e->finalized = false;
   return QD_OK;

@@ -36,20 +36,25 @@ __device__ __forceinline__ QuantK make_quantk(const qd_qparams& q) {
   return make_quantk(q.delta, q.zero_point, q.qmin, q.qmax);
 }
 
-// Exact form (7 instructions): used where the input fp32 value is itself exact w.r.t. the reference
+// y / delta with one Newton step.  When q0 = y * r overflows (y = +-inf, or |y| / delta beyond FLT_MAX) the step computes
+// fma(-inf, delta, y) = NaN, which the clamp below would turn into the LOW rail; q0 itself is then the right infinity.
+// Finite quotients never take the select, so their codes are unchanged.  NaN inputs stay NaN and clamp to the low rail.
+__device__ __forceinline__ float quant_quotient(float y, const QuantK& k) {
+  const float q0 = y * k.rdelta;
+  const float q = fmaf(fmaf(-q0, k.delta, y), k.rdelta, q0);
+  return q == q ? q : q0;
+}
+
+// Exact form (8 instructions): used where the input fp32 value is itself exact w.r.t. the reference
 // (standalone quantizer, GEMM epilogues).
 __device__ __forceinline__ uint32_t quant_code(float y, const QuantK& k) {
-  const float q0 = y * k.rdelta;
-  float q = fmaf(fmaf(-q0, k.delta, y), k.rdelta, q0);
-  q = fminf(fmaxf(q, k.flo), k.fhi);
+  const float q = fminf(fmaxf(quant_quotient(y, k), k.flo), k.fhi);
   return (uint32_t)(__float_as_int(q + 12582912.0f) - k.bias) & 0xFFu;   // rne(q) + zero_point
 }
 
 // rne(y / delta) clamped to [qmin - zp, qmax - zp]: the code minus its zero point, as a float (fp16 attention operands)
 __device__ __forceinline__ float quant_centered(float y, const QuantK& k) {
-  const float q0 = y * k.rdelta;
-  float q = fmaf(fmaf(-q0, k.delta, y), k.rdelta, q0);
-  q = fminf(fmaxf(q, k.flo), k.fhi);
+  const float q = fminf(fmaxf(quant_quotient(y, k), k.flo), k.fhi);
   return (q + 12582912.0f) - 12582912.0f;
 }
 

@@ -267,11 +267,11 @@ def _sms():
 def _launch(desc, outs):
     """One qd_qgemm_i8 call under torch.profiler; returns the (MODE, W4) pairs and whether splitk_finish_kernel ran.  The
     profiler occasionally records no kernel for a call this short; the output buffers (which may also be the residual)
-    are then restored and the call repeated, at most 3 times."""
+    are then restored and the call repeated, at most 6 times."""
     from torch.profiler import ProfilerActivity, profile
     from qdiff_b200 import ops
     saved = [t.clone() for t in outs]
-    for _ in range(3):
+    for _ in range(6):
         with profile(activities=[ProfilerActivity.CPU, ProfilerActivity.CUDA]) as prof:
             ops.qgemm(desc)
             torch.cuda.synchronize()
