@@ -22,18 +22,13 @@ the remainder.  `precision` picks the plane products that are formed:
 as 1 / 2 / 3 accumulating launches over the leading 1 / 2 / 3 activation planes (qd_gemm_desc.lda = plane pitch).
 GroupNorm + swish, the attention softmax and all accumulations are fp32.
 """
-import ctypes as C
 import os
 
 import torch
 import torch.nn as nn
 
-from . import _lib, graph, ops
-from ._lib import check, lib
+from . import _lib, graph
 from .unet import AttnBlock, _NoForward, _gn
-
-_PASSES = {1: ((0, 1),), 3: ((0, 2), (1, 1)), 6: ((0, 3), (1, 2), (2, 1))}      # (weight plane, leading activation planes)
-
 
 # ------------------------------------------------------------------------------- parameter containers
 class ResnetBlock(_NoForward):
@@ -107,8 +102,8 @@ class _FirstStage(_NoForward):
     weight_quant_params = {"n_bits": 32}
 
     def _init_engine_state(self, precision, cuda_graph):
-        if precision not in _PASSES:
-            raise ValueError(f"precision must be one of {sorted(_PASSES)} (bfloat16 plane products per MAC)")
+        if precision not in graph._PASSES:
+            raise ValueError(f"precision must be one of {sorted(graph._PASSES)} (bfloat16 plane products per MAC)")
         self.precision, self.cuda_graph = precision, cuda_graph
         self._programs, self._wcache = {}, {}
 
@@ -184,85 +179,11 @@ class FirstStageBuilder(graph.WeightOnlyBuilder):
 
     def __init__(self, fs, device, batch, precision):
         super().__init__(fs, device, batch)
-        self.passes = _PASSES[precision]
-
-    def _planes(self, conv, label, Cp, im2col):
-        """bfloat16 planes of a conv weight as GEMM operands, one tile per pass: [Np, taps, planes, Cp] with the pass's
-        weight plane repeated over the activation planes it multiplies (im2col inputs interleave the planes per tap, so
-        they always carry three plane slots, the unused ones zero)."""
-        key = (self.dev.index or 0, "fs", label, Cp, self.passes, bool(im2col))
-        ent = self.wcache.get(key)
-        if ent is not None:
-            return ent
-        w = conv.weight.detach().to(self.dev, torch.float32)
-        N, Cin = w.shape[0], w.shape[1]
-        taps = 9 if (w.dim() == 4 and w.shape[-1] == 3) else 1
-        w3 = w.reshape(N, Cin, taps).permute(0, 2, 1).contiguous()                 # [N, taps, C]
-        hi = w3.to(torch.bfloat16)
-        r1 = w3 - hi.float()
-        mid = r1.to(torch.bfloat16)
-        lo = (r1 - mid.float()).to(torch.bfloat16)
-        planes = (hi, mid, lo)
-        Np = (N + 3) // 4 * 4              # the specialised epilogues store 4 columns at a time (conv_out: 3 channels)
-        tiles = []
-        for wp, nact in self.passes:
-            slots = 3 if im2col else nact
-            wk = torch.zeros((Np, taps, slots, Cp), dtype=torch.bfloat16, device=self.dev)
-            wk[:N, :, :nact, :Cin] = planes[wp][:, :, None, :]
-            tiles.append((wk.reshape(Np, -1).contiguous(), slots))
-        bias = torch.zeros(Np, dtype=torch.float32, device=self.dev)
-        if conv.bias is not None:
-            bias[:N] = conv.bias.detach().to(self.dev, torch.float32)
-        ent = dict(tiles=tiles, N=Np, N_real=N, taps=taps, bias=bias, ones=torch.ones(Np, dtype=torch.float32, device=self.dev))
-        self.wcache[key] = ent
-        return ent
-
-    def gemm_fp(self, conv, a, label, *, hw=None, residual=None, im2col=None):
-        """One floating-point conv / 1x1 conv: len(self.passes) accumulating GEMM launches.  a: split3 planes of the input.
-        hw: 3x3 stride-1 conv on an (H, W) map (implicit GEMM); im2col = (hw, stride, pad_tl, out_hw): explicit patches."""
-        if im2col is None and hw is not None and int(conv.weight.shape[-1]) == 3 and not self.implicit_conv_ok(hw[0], hw[1]):
-            im2col = (hw, 1, (1, 1), hw)          # feature-map sizes the implicit-GEMM tiling does not cover
-        W = self._planes(conv, label, a.Cp, im2col is not None)
-        N, taps = W["N"], W["taps"]
-        self.keep += [W["bias"], W["ones"]] + [t for t, _ in W["tiles"]]
-        src, conv_bhw, rows_pb = a, None, 0
-        if im2col is not None:
-            (H, Wd), stride, pad_tl, (Ho, Wo) = im2col
-            cbytes = 6 * a.Cp
-            patches = torch.zeros((self.B * Ho * Wo, 9 * cbytes), dtype=torch.uint8, device=self.dev)
-            self.keep.append(patches)
-            di = ops.im2col_desc(a.t, patches, B=self.B, H=H, W=Wd, C_=cbytes, Ho=Ho, Wo=Wo, stride=stride,
-                                 pad_top=pad_tl[0], pad_left=pad_tl[1], pad_code=0, ld_dst=9 * cbytes)
-            src = graph.Act(patches, self.B * Ho * Wo, 9 * cbytes)
-            self.add(_lib.QD_OP_IM2COL, di, label + ".im2col")
-        elif taps == 9:
-            conv_bhw, rows_pb = (self.B, hw[0], hw[1]), hw[0] * hw[1]
-        M = src.rows
-        o = self.new_f32(M, N)
-        for i, (tile, slots) in enumerate(W["tiles"]):
-            if im2col is not None:
-                g_taps, g_c, lda = 1, 9 * 6 * a.Cp, 9 * 6 * a.Cp
-            else:
-                g_taps, g_c, lda = taps, 2 * slots * a.Cp, 6 * a.Cp            # bytes: leading `slots` planes of 3
-            res = residual if i == 0 else o
-            d = ops.gemm_desc(src.t, tile, W["ones"], M=M, N=N, C=g_c, taps=g_taps, lda=lda, conv_bhw=conv_bhw,
-                              a_signed=False, bias=W["bias"] if i == 0 else None, rows_per_batch=rows_pb,
-                              residual=res.t if res is not None else None, ldr=res.ld if res is not None else 0,
-                              out=o.t, ldo=o.ld)
-            d.a_bf16 = 1
-            d.a = src.ptr
-            if res is not None:
-                d.residual = res.ptr
-            d.out = o.ptr
-            Cin = int(conv.weight.shape[1])
-            self.add(_lib.QD_OP_GEMM, d, label + (f".pass{i}" if i else ""),
-                     flops=2 * M * W["N_real"] * Cin * taps if i == 0 else 0)
-        self.layer_traces[label] = o
-        return o
+        self.precision = precision
 
     def conv(self, conv, x_f32, label, hw, residual=None, upsample=None):
         a = self.split3(x_f32, label + ".split", upsample=upsample)
-        return self.gemm_fp(conv, a, label, hw=hw, residual=residual)
+        return self.plane_gemm(conv, a, label, hw=hw, residual=residual)
 
     def resnet(self, blk, x, hw):
         """ResnetBlock.forward (model.py:122-144), temb None."""
@@ -286,9 +207,9 @@ class FirstStageBuilder(graph.WeightOnlyBuilder):
         T, C_ = hw[0] * hw[1], x.cols
         hn = self.gn_f32(x, blk.norm, T, False, k + ".norm")
         a = self.split3(hn, k + ".qkv.split")
-        q = self.gemm_fp(blk.q, a, k + ".q")
-        kk = self.gemm_fp(blk.k, a, k + ".k")
-        v = self.gemm_fp(blk.v, a, k + ".v")
+        q = self.plane_gemm(blk.q, a, k + ".q")
+        kk = self.plane_gemm(blk.k, a, k + ".k")
+        v = self.plane_gemm(blk.v, a, k + ".v")
         mode = os.environ.get("QDIFF_FS_ATTN", "auto")
         if (mode == "tc" or (mode == "auto" and T >= 1024)) and T % 16 == 0 and C_ % 16 == 0:
             o = self.attn_products_tc(q, kk, v, T, C_, k + ".attn")
@@ -297,8 +218,8 @@ class FirstStageBuilder(graph.WeightOnlyBuilder):
                                   scale=float(int(C_) ** (-0.5)), label=k + ".attn")
         return self.conv(blk.proj_out, o, k + ".proj_out", hw, residual=x)
 
-    def _plane_tiles(self, planes, rows, Cp, passes, label):
-        """GEMM B operands from the bfloat16 planes [rows, 3 * Cp] of a RUN-TIME matrix (K or V^T): for every pass
+    def _plane_tiles(self, planes, rows, Cp, passes, scale, label):
+        """plane_gemm operand from the bfloat16 planes [rows, 3 * Cp] of a RUN-TIME matrix (K or V^T): for every pass
         (plane, n) the tile [rows, n * Cp] = that plane repeated n times - strided 2-D copies of the planes (the planes are
         addressed as fp32 pairs: Cp % 8 == 0)."""
         tiles = []
@@ -309,19 +230,7 @@ class FirstStageBuilder(graph.WeightOnlyBuilder):
                 self.misc(_lib.QD_OP_COPY2D, planes.ptr + 2 * wp * Cp, t.data_ptr() + 2 * sl * Cp, rows, Cp // 2,
                           ld_src=3 * Cp // 2, ld_dst=nact * Cp // 2, label=f"{label}.tile{wp}.{sl}")
             tiles.append((t, nact))
-        return tiles
-
-    def _gemm_planes(self, a, tiles, scale, M, N, Cp, out, label):
-        """out[M, N] = scale[n] * sum over the passes of A-planes x tile^T (accumulating launches), fp32."""
-        for i, (tile, nact) in enumerate(tiles):
-            d = ops.gemm_desc(a.t, tile, scale, M=M, N=N, C=2 * nact * Cp, taps=1, lda=6 * Cp, a_signed=False,
-                              residual=out.t if i else None, ldr=out.ld if i else 0, out=out.t, ldo=out.ld)
-            d.a_bf16 = 1
-            d.a = a.ptr
-            if i:
-                d.residual = out.ptr
-            d.out = out.ptr
-            self.add(_lib.QD_OP_GEMM, d, label + (f".pass{i}" if i else ""), flops=2 * M * N * Cp if i == 0 else 0)
+        return dict(tiles=tiles, scale=scale, bias=None, N=rows, N_real=rows, taps=1)
 
     def attn_products_tc(self, q, k, v, T, C_, label):
         """softmax(q k^T C^-1/2) v with both products as bfloat16-plane GEMMs on wgmma (fp32 accumulation), per image:
@@ -341,14 +250,15 @@ class FirstStageBuilder(graph.WeightOnlyBuilder):
             aq = self.split3(qb, lb + ".q.split")
             pk = self.split3(kb, lb + ".k.split")
             S = self.new_f32(T, T)
-            self._gemm_planes(aq, self._plane_tiles(pk, T, aq.Cp, _PASSES[6], lb + ".k"), sc_qk, T, T, aq.Cp, S, lb + ".qk")
+            self.plane_gemm(self._plane_tiles(pk, T, aq.Cp, graph._PASSES[6], sc_qk, lb + ".k"), aq, lb + ".qk", out=S)
             self.misc(_lib.QD_OP_SOFTMAX_ROWS, S.ptr, S.ptr, T, T, ld_src=S.ld, ld_dst=S.ld, label=lb + ".softmax")
             ap = self.split3(S, lb + ".p.split")
             vt = self.new_f32(C_, T)
             self.misc(_lib.QD_OP_NHWC_TO_NCHW, self.contig(vb, lb + ".v").ptr, vt.ptr, 1, C_, T, label=lb + ".v.t")
             pv = self.split3(vt, lb + ".vt.split")
             ob = graph.Act(o_all.t[rows], T, C_, ld=o_all.ld)
-            self._gemm_planes(ap, self._plane_tiles(pv, C_, ap.Cp, self.passes, lb + ".vt"), ones_c, T, C_, ap.Cp, ob, lb + ".pv")
+            self.plane_gemm(self._plane_tiles(pv, C_, ap.Cp, graph._PASSES[self.precision], ones_c, lb + ".vt"), ap, lb + ".pv",
+                            out=ob)
         return o_all
 
     def lower(self, fs, z_shape, quantize):
@@ -370,7 +280,7 @@ class FirstStageBuilder(graph.WeightOnlyBuilder):
         hw = (H, W)
         h = self.conv(fs.post_quant_conv, zh, "post_quant_conv", hw)
         h = h.view(0, int(fs.post_quant_conv.weight.shape[0]))              # drop the padding columns (N rounded up to 4)
-        h = self.gemm_fp(dec.conv_in, self.split3(h, "decoder.conv_in.split"), "decoder.conv_in", im2col=(hw, 1, (1, 1), hw))
+        h = self.plane_gemm(dec.conv_in, self.split3(h, "decoder.conv_in.split"), "decoder.conv_in", im2col=(hw, 1, (1, 1), hw))
         h = self.resnet(dec.mid.block_1, h, hw)
         h = self.attn(dec.mid.attn_1, h, hw)
         h = self.resnet(dec.mid.block_2, h, hw)
@@ -386,7 +296,7 @@ class FirstStageBuilder(graph.WeightOnlyBuilder):
                 if up.with_conv:
                     a = self.split3(h, self.key(up.conv) + ".split", upsample=(B, hw[0], hw[1]))
                     hw = (2 * hw[0], 2 * hw[1])
-                    h = self.gemm_fp(up.conv, a, self.key(up.conv), hw=hw)
+                    h = self.plane_gemm(up.conv, a, self.key(up.conv), hw=hw)
                 else:
                     big = self.new_f32(4 * h.rows, h.cols)
                     self.misc(_lib.QD_OP_UPSAMPLE2X, self.contig(h, "up").ptr, big.ptr, B, hw[0], hw[1], h.cols,
@@ -403,18 +313,10 @@ class FirstStageBuilder(graph.WeightOnlyBuilder):
 
 def compile_decoder(fs, z_shape, device, quantize=False, precision=3, use_cuda_graph=True):
     """Lower the decode step of `fs` (AutoencoderKL / VQModelInterface container) for a fixed latent shape."""
-    lib()       # fail loudly if the CUDA library is missing
-    if not torch.cuda.is_available():
-        raise RuntimeError("qdiff_b200: no CUDA device; the engine has no CPU fallback")
     b = FirstStageBuilder(fs, device, z_shape[0], precision)
     with torch.no_grad():
         x_in, t_in, out = b.lower(fs, z_shape, quantize)
-    b.flush()
-    check(lib().qd_engine_finalize(b.engine), "qd_engine_finalize")
-    prog = graph.Program(b.engine, b.keep, x_in, t_in, None, out, b.nops, b.traces, use_cuda_graph)
-    prog.op_names, prog.op_kinds, prog.op_flops = b.op_names, b.op_kinds, b.op_flops
-    prog.layer_traces = b.layer_traces
-    return prog
+    return b.finish(graph.Program, x_in, t_in, None, out, use_cuda_graph)
 
 
 # first-stage hyper-parameters of the reference's configs (configs/stable-diffusion/v1-inference.yaml:46-67,

@@ -60,12 +60,12 @@ class _Offset:
 
 class Program:
     """A compiled UNet: ops [0, n_static) depend only on the cross-attention context (replayed when it changes),
-    ops [n_static, nops) are the per-step program.  Each range is captured as one CUDA graph."""
+    ops [n_static, nops) are the per-step program.  Each range is captured as one CUDA graph.  Built by Builder.finish,
+    which also sets nops, n_static and the recorded metadata."""
 
-    def __init__(self, engine, keep, x_in, t_in, ctx_in, out, nops, traces, use_cuda_graph, n_static=0):
+    def __init__(self, engine, keep, x_in, t_in, ctx_in, out, use_cuda_graph):
         self.engine, self.keep = engine, keep
         self.x_in, self.t_in, self.ctx_in, self.out = x_in, t_in, ctx_in, out
-        self.nops, self.traces, self.n_static = nops, traces, n_static
         self.use_cuda_graph = use_cuda_graph
         self.graph = None
         self.graph_static = None
@@ -147,7 +147,9 @@ class Builder:
     def __init__(self, qnn, device, batch):
         self.qnn, self.dev, self.B = qnn, device, batch
         self.names = {id(m): n for n, m in qnn.named_modules()}
-        e = C.c_void_p()
+        if not torch.cuda.is_available():
+            raise RuntimeError("qdiff_b200: no CUDA device; the engine has no CPU fallback")
+        e = C.c_void_p()    # lib() fails loudly if the CUDA library is missing
         check(lib().qd_engine_create(device.index or 0, C.byref(e)), "qd_engine_create")
         self.engine = e
         self.keep = []       # tensors referenced by recorded ops
@@ -261,6 +263,17 @@ class Builder:
             self.op_flops.append(flops)
             self.op_specs.append(spec)
         self._pending = []
+
+    def finish(self, program_cls, *args):
+        """The compile tail of every lowering: hand the recorded ops to the engine, finalise it, and wrap it in
+        program_cls(engine, keep, *args) carrying the recorded metadata."""
+        self.flush()
+        check(lib().qd_engine_finalize(self.engine), "qd_engine_finalize")
+        prog = program_cls(self.engine, self.keep, *args)
+        prog.nops, prog.n_static, prog.traces, prog.layer_traces = self.nops, self.n_static, self.traces, self.layer_traces
+        prog.op_names, prog.op_kinds, prog.op_flops, prog.op_specs = self.op_names, self.op_kinds, self.op_flops, self.op_specs
+        prog.kernel_launches = sum(3 if k == _lib.QD_OP_GROUPNORM else 1 for k in self.op_kinds[self.n_static:])  # until run
+        return prog
 
     @staticmethod
     def _covered(ranges, lo, hi):
@@ -1179,7 +1192,13 @@ class Builder:
         return x_in, t_in, None, out
 
 
-# ====================================================================== weight-only lowering (quant_act False)
+# ====================================================================== bfloat16-plane lowering (quant_act False)
+# (weight plane, leading activation planes) of each accumulating launch, by the bfloat16 plane products formed per MAC:
+# 1 = x_hi w_hi;  3 adds x_mid w_hi + x_hi w_mid;  6 adds x_lo w_hi + x_mid w_mid + x_hi w_lo (fp32-faithful: 2^-24)
+_PASSES = {1: ((0, 1),), 3: ((0, 2), (1, 1)), 6: ((0, 3), (1, 2), (2, 1))}
+_CODES = ((None, 3),)       # integer weight codes, exact in bfloat16: one launch against all three activation planes
+
+
 class WeightOnlyBuilder(Builder):
     """set_quant_state(True, False): quantised weights, fp32 activations (BASELINE configs[0], qdiff/utils.py:407), and
     set_quant_state(False, False): the full-precision state the reference uses for FP baselines and calibration data.
@@ -1189,7 +1208,10 @@ class WeightOnlyBuilder(Builder):
     contraction with fp32 accumulation, i.e. the reference's fp32 conv up to summation order.  With use_weight_quant
     False the fp32 weight is split into three bfloat16 planes as well and the six plane products down to 2^-24 are formed
     in three accumulating launches (x_{hi,mid,lo} w_hi, x_{hi,mid} w_mid, x_hi w_lo: qd_gemm_desc.lda = plane pitch).
-    Norms emit fp32 (+SiLU), attention runs in fp32 (qd_attention_fp32).  Families: ddim (CIFAR), LDM and SD UNets."""
+    Norms emit fp32 (+SiLU), attention runs in fp32 (qd_attention_fp32).  Families: ddim (CIFAR), LDM and SD UNets.
+    The first stage and the text encoder lower their floating-point GEMMs through the same recorder (plane_gemm)."""
+
+    precision = None    # plane products of fp32 weights (_PASSES); None: each QuantModule's state picks codes or six
 
     def split3(self, src, label, act=0, upsample=None, cols=None):
         C_ = src.cols if cols is None else cols
@@ -1204,161 +1226,122 @@ class WeightOnlyBuilder(Builder):
         self.add(_lib.QD_OP_SPLIT3, d, label, spec=dict(kind="split3", src=src, dst=a, act=act, upsample=upsample, C=C_, Cp=Cp))
         return a
 
-    def gemm_wo(self, qm, a, label, *, conv_bhw=None, rowvec=None, residual=None, out=None, rows_per_batch=0, cols=None,
-                suffix="", accumulate_into=None, use_bias=True, im2col=None):
-        """One weight-only GEMM.  a: bfloat16 plane Act from split3.  im2col = (hw, stride, pad_tl, out_hw): explicit patch
-        gather first (strided convs, conv_in)."""
-        cols = tuple(cols) if cols is not None else None
-        if conv_bhw is not None and im2col is None and not self.implicit_conv_ok(conv_bhw[1], conv_bhw[2]):
-            hw_ = (conv_bhw[1], conv_bhw[2])
-            conv_bhw, im2col = None, (hw_, 1, (1, 1), hw_)          # any feature-map size: explicit patch gather
-        if not getattr(qm, "use_weight_quant", True):
-            return self._gemm_fp_weights(qm, a, label, conv_bhw=conv_bhw, rowvec=rowvec, residual=residual, out=out,
-                                         rows_per_batch=rows_per_batch, cols=cols, accumulate_into=accumulate_into,
-                                         use_bias=use_bias, im2col=im2col)
-        key = (self.dev.index or 0, "wo", label, cols, suffix, conv_bhw is not None or im2col is not None)
+    def plane_weights(self, qm, label, Cp, passes, im2col, cols=None, suffix=""):
+        """The weight operand of a bfloat16-plane GEMM, shared by every program of the model and keyed by the op label.
+        One tile [Np, taps, slots, Cp] bf16 per pass: the pass's weight plane repeated over the activation planes it
+        multiplies, N padded to 4 columns (the specialised epilogues store 4 at a time: conv_out has 3 channels).  Patches
+        (im2col) interleave all three activation planes per tap, so their tiles have three slots, the unused ones zero.
+        Integer codes (passes _CODES) carry the per-channel step delta_w as scale, fp32 weights scale 1.  The padded bias
+        is read from the module on first use (an engine-native checkpoint restores it with the model: packed.py)."""
+        slots = tuple(3 if im2col else n for _, n in passes)
+        key = (self.dev.index or 0, "planes", label, cols, suffix, passes, slots)
         ent = self.wcache.get(key)
-        if ent is None or (self.want_specs and "ws_cpu" not in ent):
-            ws, delta_w = self._fold(qm, cols, suffix)
-            N = ws.shape[0]
-            taps = 9 if (ws.dim() == 4 and ws.shape[-1] == 3) else 1
-            w3 = ws.reshape(N, ws.shape[1], taps).permute(0, 2, 1)                  # [N, taps, C]
-            Np = (N + 3) // 4 * 4          # the specialised epilogues store 4 columns at a time: pad conv_out (3 channels)
-            wk = torch.zeros((Np, taps, 3, a.Cp), dtype=torch.bfloat16, device=self.dev)
-            wk[:N, :, :, :ws.shape[1]] = w3.to(torch.bfloat16)[:, :, None, :]
-            dw = torch.ones(Np, dtype=torch.float32, device=self.dev)
-            dw[:N] = delta_w.to(torch.float32)
-            ent = dict(w_dev=wk.reshape(Np, -1).contiguous(), delta_w=dw, N=Np, N_real=N, taps=taps)
-            if self.want_specs:
-                wpad = torch.zeros((Np,) + tuple(ws.shape[1:]), dtype=torch.float32)
-                wpad[:N] = ws.detach().to("cpu", torch.float32)
-                ent["ws_cpu"] = wpad
-            self.wcache[key] = ent
-        N, taps, w_dev, scale = ent["N"], ent["taps"], ent["w_dev"], ent["delta_w"]
-        self.keep += [w_dev, scale]
-        bias = None
-        if use_bias and qm.bias is not None:
-            bias = torch.zeros(N, dtype=torch.float32, device=self.dev)
-            bias[:ent["N_real"]] = qm.bias.detach().to(self.dev, torch.float32)
-            self.keep.append(bias)
-        cbytes = 6 * a.Cp
-        src_act = a
-        if im2col is not None:
-            (H, W), stride, pad_tl, (Ho, Wo) = im2col
-            patches = torch.zeros((self.B * Ho * Wo, 9 * cbytes), dtype=torch.uint8, device=self.dev)
-            self.keep.append(patches)
-            di = ops.im2col_desc(a.t, patches, B=self.B, H=H, W=W, C_=cbytes, Ho=Ho, Wo=Wo, stride=stride,
-                                 pad_top=pad_tl[0], pad_left=pad_tl[1], pad_code=0, ld_dst=9 * cbytes)
-            pa = Act(patches, self.B * Ho * Wo, 9 * cbytes)
-            pa.bf16, pa.C, pa.Cp = True, a.C, a.Cp
-            self.add(_lib.QD_OP_IM2COL, di, label + ".im2col",
-                     spec=dict(kind="im2col_bytes", src=a, dst=pa, B=self.B, H=H, W=W, Ho=Ho, Wo=Wo, stride=stride,
-                               pad_tl=pad_tl, cbytes=cbytes))
-            src_act, gemm_taps, gemm_c, conv_bhw = pa, 1, 9 * cbytes, None
-        elif taps == 9:
-            gemm_taps, gemm_c = 9, cbytes
-        else:
-            gemm_taps, gemm_c = 1, cbytes
-        M = src_act.rows
-        o = accumulate_into if accumulate_into is not None else (out if out is not None else self.new_f32(M, N))
-        res = accumulate_into if accumulate_into is not None else residual
-        d = ops.gemm_desc(src_act.t, w_dev, scale, M=M, N=N, C=gemm_c, taps=gemm_taps, lda=src_act.ld * src_act.t.element_size(),
-                          conv_bhw=conv_bhw, a_signed=False, bias=bias,
-                          rowvec=rowvec.t if rowvec is not None else None, ld_rowvec=rowvec.ld if rowvec is not None else 0,
-                          rows_per_batch=rows_per_batch, residual=res.t if res is not None else None,
-                          ldr=res.ld if res is not None else 0, out=o.t, ldo=o.ld)
-        d.a_bf16 = 1
-        d.a = src_act.ptr
-        if rowvec is not None:
-            d.rowvec = rowvec.ptr
-        if res is not None:
-            d.residual = res.ptr
-        d.out = o.ptr
-        spec = None
-        if self.want_specs:
-            spec = dict(kind="gemm_wo", key=self.key(qm) if id(qm) in self.names else self.key(qm.qm), a=src_act, Cp=a.Cp,
-                        C=a.C, taps=9 if (taps == 9) else 1, im2col=im2col is not None, conv_bhw=conv_bhw, ws=ent["ws_cpu"],
-                        scale=scale.detach().cpu(), bias=None if bias is None else bias.detach().cpu(), rowvec=rowvec,
-                        residual=res, rows_per_batch=rows_per_batch, out=o, N=N)
-        self.add(_lib.QD_OP_GEMM, d, label, flops=2 * M * N * (gemm_c // 6) * gemm_taps, spec=spec)
-        self.layer_traces[label] = o
-        return o
-
-    def _gemm_fp_weights(self, qm, a, label, *, conv_bhw, rowvec, residual, out, rows_per_batch, cols, accumulate_into,
-                         use_bias, im2col):
-        """use_weight_quant False: the layer's fp32 weight as three bfloat16 planes; launches (weight plane, leading
-        activation planes) = (hi, 3), (mid, 2), (lo, 1), each accumulating into the first one's output."""
-        key = (self.dev.index or 0, "wofp", label, cols, im2col is not None)
-        ent = self.wcache.get(key)
-        if ent is None:
-            w = qm.weight.detach().to(self.dev, torch.float32)
-            if cols is not None:
-                w = w[:, cols[0]:cols[1], ...]
+        if ent is None or (self.want_specs and passes is _CODES and "ws_cpu" not in ent):
+            if passes is _CODES:
+                w, delta_w = self._fold(qm, cols, suffix)
+                planes = (w.to(torch.bfloat16),)
+            else:
+                w = qm.weight.detach().to(self.dev, torch.float32)
+                w = w if cols is None else w[:, cols[0]:cols[1], ...]
+                hi = w.to(torch.bfloat16)
+                r1 = w - hi.float()
+                mid = r1.to(torch.bfloat16)
+                planes = (hi, mid, (r1 - mid.float()).to(torch.bfloat16))
             N, Cin = w.shape[0], w.shape[1]
             taps = 9 if (w.dim() == 4 and w.shape[-1] == 3) else 1
-            w3 = w.reshape(N, Cin, taps).permute(0, 2, 1).contiguous()
-            hi = w3.to(torch.bfloat16)
-            r1 = w3 - hi.float()
-            mid = r1.to(torch.bfloat16)
-            lo = (r1 - mid.float()).to(torch.bfloat16)
             Np = (N + 3) // 4 * 4
             tiles = []
-            for plane, nact in ((hi, 3), (mid, 2), (lo, 1)):
-                slots = 3 if im2col is not None else nact       # im2col patches interleave the planes per tap
-                wk = torch.zeros((Np, taps, slots, a.Cp), dtype=torch.bfloat16, device=self.dev)
-                wk[:N, :, :nact, :Cin] = plane[:, :, None, :]
-                tiles.append((wk.reshape(Np, -1).contiguous(), slots))
-            ent = dict(tiles=tiles, N=Np, N_real=N, taps=taps, ones=torch.ones(Np, dtype=torch.float32, device=self.dev))
+            for (wp, nact), s in zip(passes, slots):
+                wk = torch.zeros((Np, taps, s, Cp), dtype=torch.bfloat16, device=self.dev)
+                wk[:N, :, :nact, :Cin] = planes[wp or 0].reshape(N, Cin, taps).permute(0, 2, 1)[:, :, None, :]
+                tiles.append((wk.reshape(Np, -1).contiguous(), s))
+            scale = torch.ones(Np, dtype=torch.float32, device=self.dev)
+            ent = dict(tiles=tiles, scale=scale, N=Np, N_real=N, taps=taps)
+            if passes is _CODES:
+                scale[:N] = delta_w.to(torch.float32)
+                if self.want_specs:
+                    ent["ws_cpu"] = torch.zeros((Np,) + tuple(w.shape[1:]), dtype=torch.float32)
+                    ent["ws_cpu"][:N] = w.detach().to("cpu", torch.float32)
             self.wcache[key] = ent
-        N, taps = ent["N"], ent["taps"]
-        self.keep += [ent["ones"]] + [t for t, _ in ent["tiles"]]
-        bias = None
-        if use_bias and qm.bias is not None:
-            bias = torch.zeros(N, dtype=torch.float32, device=self.dev)
-            bias[:ent["N_real"]] = qm.bias.detach().to(self.dev, torch.float32)
-            self.keep.append(bias)
-        src_act = a
+        if "bias" not in ent:
+            b = qm.bias
+            ent["bias"] = None if b is None else \
+                torch.nn.functional.pad(b.detach().to(self.dev, torch.float32), (0, ent["N"] - ent["N_real"]))
+        return ent
+
+    def plane_gemm(self, op, a, label, *, hw=None, im2col=None, rows_per_batch=None, rowvec=None, residual=None,
+                   out=None, accumulate_into=None, use_bias=True, cols=None, suffix=""):
+        """Record y = x W^T [+ bias] [+ rowvec] [+ residual] on the bfloat16 planes `a` of x (split3): one accumulating
+        launch per pass of the weight operand; the first carries bias, rowvec and the residual (or accumulate_into's
+        contents), the later ones add into its output.
+        op: a module (its weight through plane_weights; cols / suffix pick a column range and its quantizer, for the
+        split-shortcut halves and K slices), or a run-time operand dict of the same shape (_plane_tiles).
+        hw = (H, W): a 3x3 stride-1 conv on that map - the implicit GEMM where the map tiles, else the patch gather;
+        im2col = (hw, stride, pad_tl, out_hw): the patch gather always (strided convs, conv_in).
+        rows_per_batch (rows per image, for rowvec) defaults to H*W for the implicit conv, else 0."""
+        cols = tuple(cols) if cols is not None else None
+        if im2col is None and hw is not None and int(op.weight.shape[-1]) == 3 and not self.implicit_conv_ok(*hw):
+            im2col = (hw, 1, (1, 1), hw)          # e.g. 96x96 or 24x24 latents: correct for any size, 9x the operand bytes
+        codes = False
+        if isinstance(op, dict):
+            W = op
+        else:
+            codes = self.precision is None and getattr(op, "use_weight_quant", True)
+            passes = _CODES if codes else _PASSES[self.precision or 6]
+            W = self.plane_weights(op, label, a.Cp, passes, im2col is not None, cols=cols, suffix=suffix)
+        N, taps, scale = W["N"], W["taps"], W["scale"]
+        bias = W["bias"] if use_bias else None
+        self.keep += [scale] + [t for t, _ in W["tiles"]] + ([bias] if bias is not None else [])
+        src, conv_bhw = a, None
         if im2col is not None:
-            (H, W), stride, pad_tl, (Ho, Wo) = im2col
+            (H, Wd), stride, pad_tl, (Ho, Wo) = im2col
             cbytes = 6 * a.Cp
             patches = torch.zeros((self.B * Ho * Wo, 9 * cbytes), dtype=torch.uint8, device=self.dev)
             self.keep.append(patches)
-            di = ops.im2col_desc(a.t, patches, B=self.B, H=H, W=W, C_=cbytes, Ho=Ho, Wo=Wo, stride=stride,
+            src = Act(patches, self.B * Ho * Wo, 9 * cbytes)
+            src.bf16, src.C, src.Cp = True, a.C, a.Cp
+            di = ops.im2col_desc(a.t, patches, B=self.B, H=H, W=Wd, C_=cbytes, Ho=Ho, Wo=Wo, stride=stride,
                                  pad_top=pad_tl[0], pad_left=pad_tl[1], pad_code=0, ld_dst=9 * cbytes)
-            src_act = Act(patches, self.B * Ho * Wo, 9 * cbytes)
-            src_act.bf16, src_act.C, src_act.Cp = True, a.C, a.Cp
-            self.add(_lib.QD_OP_IM2COL, di, label + ".im2col")
-            conv_bhw = None
-        M = src_act.rows
+            self.add(_lib.QD_OP_IM2COL, di, label + ".im2col",
+                     spec=dict(kind="im2col_bytes", src=a, dst=src, B=self.B, H=H, W=Wd, Ho=Ho, Wo=Wo, stride=stride,
+                               pad_tl=pad_tl, cbytes=cbytes) if codes else None)
+        elif hw is not None and taps == 9:
+            conv_bhw = (self.B, hw[0], hw[1])
+        if rows_per_batch is None:
+            rows_per_batch = hw[0] * hw[1] if conv_bhw is not None else 0
+        M = src.rows
         o = accumulate_into if accumulate_into is not None else (out if out is not None else self.new_f32(M, N))
-        first_res = accumulate_into if accumulate_into is not None else residual
-        for i, (tile, slots) in enumerate(ent["tiles"]):
-            if im2col is not None:
-                g_taps, g_c, lda = 1, 9 * 6 * a.Cp, 9 * 6 * a.Cp
-            else:
-                g_taps, g_c, lda = taps, 2 * slots * a.Cp, src_act.ld * src_act.t.element_size()
-            res = first_res if i == 0 else o
-            rv = rowvec if i == 0 else None
-            d = ops.gemm_desc(src_act.t, tile, ent["ones"], M=M, N=N, C=g_c, taps=g_taps, lda=lda, conv_bhw=conv_bhw,
+        res = accumulate_into if accumulate_into is not None else residual
+        spec = None
+        if codes and self.want_specs:
+            spec = dict(kind="gemm_wo", key=self.key(op) if id(op) in self.names else self.key(op.qm), a=src, Cp=a.Cp,
+                        C=a.C, taps=taps, im2col=im2col is not None, conv_bhw=conv_bhw, ws=W["ws_cpu"],
+                        scale=scale.detach().cpu(), bias=None if bias is None else bias.detach().cpu(), rowvec=rowvec,
+                        residual=res, rows_per_batch=rows_per_batch, out=o, N=N)
+        for i, (tile, slots) in enumerate(W["tiles"]):
+            if i:
+                rowvec, res = None, o
+            d = ops.gemm_desc(src.t, tile, scale, M=M, N=N, C=2 * slots * a.Cp * (9 if im2col else 1),
+                              taps=1 if im2col else taps, lda=src.ld * src.t.element_size(), conv_bhw=conv_bhw,
                               a_signed=False, bias=bias if i == 0 else None,
-                              rowvec=rv.t if rv is not None else None, ld_rowvec=rv.ld if rv is not None else 0,
+                              rowvec=rowvec.t if rowvec is not None else None, ld_rowvec=rowvec.ld if rowvec is not None else 0,
                               rows_per_batch=rows_per_batch, residual=res.t if res is not None else None,
                               ldr=res.ld if res is not None else 0, out=o.t, ldo=o.ld)
             d.a_bf16 = 1
-            d.a = src_act.ptr
-            if rv is not None:
-                d.rowvec = rv.ptr
+            d.a = src.ptr
+            if rowvec is not None:
+                d.rowvec = rowvec.ptr
             if res is not None:
                 d.residual = res.ptr
             d.out = o.ptr
-            Cin = int(qm.weight.shape[1]) if cols is None else cols[1] - cols[0]
-            self.add(_lib.QD_OP_GEMM, d, label + (f".pass{i}" if i else ""), flops=2 * M * ent["N_real"] * Cin * taps if i == 0 else 0)
+            self.add(_lib.QD_OP_GEMM, d, label + (f".pass{i}" if i else ""),
+                     flops=0 if i else 2 * M * W["N_real"] * a.C * taps, spec=None if i else spec)
         self.layer_traces[label] = o
         return o
 
     def lin(self, qm, x_f32, label, act=0, **kw):
         cols = x_f32.cols // 2 if act == 2 else None
-        return self.gemm_wo(qm, self.split3(x_f32, label + ".split", act=act, cols=cols), label, **kw)
+        return self.plane_gemm(qm, self.split3(x_f32, label + ".split", act=act, cols=cols), label, **kw)
 
     def ln_f32(self, x, norm, label):
         """nn.LayerNorm with fp32 output (qd_layernorm_quant, n_out = 0)."""
@@ -1397,8 +1380,8 @@ class WeightOnlyBuilder(Builder):
         if split and getattr(qm, "use_weight_quant", True):     # full precision: the split only affects quantizers
             if qm.split == 0:
                 raise RuntimeError(f"{label}: split is set but the checkpoint has no split quantizers")
-            s = self.gemm_wo(qm, self.split3(x.view(0, split), label + ".split0"), label + ".half0", cols=(0, split))
-            self.gemm_wo(qm, self.split3(x.view(split, x.cols - split), label + ".split1"), label, cols=(split, x.cols),
+            s = self.plane_gemm(qm, self.split3(x.view(0, split), label + ".split0"), label + ".half0", cols=(0, split))
+            self.plane_gemm(qm, self.split3(x.view(split, x.cols - split), label + ".split1"), label, cols=(split, x.cols),
                          suffix="_0", accumulate_into=s, use_bias=False)
             return s
         return self.lin(qm, x, label)
@@ -1410,7 +1393,7 @@ class WeightOnlyBuilder(Builder):
         H, W = hw
         h1 = self.gn_f32(x, blk.norm1, H * W, True, k + ".norm1")
         tp = self.lin(blk.temb_proj, temb, k + ".temb_proj", act=1)
-        h = self.gemm_wo(blk.conv1, self.split3(h1, k + ".conv1.split"), k + ".conv1", conv_bhw=(self.B, H, W),
+        h = self.plane_gemm(blk.conv1, self.split3(h1, k + ".conv1.split"), k + ".conv1", hw=(H, W),
                          rows_per_batch=H * W, rowvec=tp)
         h2 = self.gn_f32(h, blk.norm2, H * W, True, k + ".norm2")
         s = x
@@ -1418,7 +1401,7 @@ class WeightOnlyBuilder(Builder):
             if getattr(blk, "use_conv_shortcut", False):
                 raise NotImplementedError("conv_shortcut=True is not used by the reference configs")
             s = self.shortcut(blk.nin_shortcut, x, k + ".nin_shortcut", split)
-        return self.gemm_wo(blk.conv2, self.split3(h2, k + ".conv2.split"), k + ".conv2", conv_bhw=(self.B, H, W),
+        return self.plane_gemm(blk.conv2, self.split3(h2, k + ".conv2.split"), k + ".conv2", hw=(H, W),
                             rows_per_batch=H * W, residual=s)
 
     def ddim_attn(self, blk, x, hw):
@@ -1428,9 +1411,9 @@ class WeightOnlyBuilder(Builder):
         C_ = x.cols
         hn = self.gn_f32(x, blk.norm, T, False, k + ".norm")
         a = self.split3(hn, k + ".qkv.split")
-        q = self.gemm_wo(blk.q, a, k + ".q")
-        kk = self.gemm_wo(blk.k, a, k + ".k")
-        v = self.gemm_wo(blk.v, a, k + ".v")
+        q = self.plane_gemm(blk.q, a, k + ".q")
+        kk = self.plane_gemm(blk.k, a, k + ".k")
+        v = self.plane_gemm(blk.v, a, k + ".v")
         o = self.attention_fp(q, kk, v, heads=1, d=C_, Tq=T, Tk=T, q_layout=(0, C_), k_layout=(0, C_), v_layout=(0, C_),
                               scale=float(int(C_) ** (-0.5)), label=k + ".attn")
         return self.lin(blk.proj_out, o, k + ".proj_out", residual=x)
@@ -1450,7 +1433,7 @@ class WeightOnlyBuilder(Builder):
         self.misc(_lib.QD_OP_NCHW_TO_NHWC, x_in.data_ptr(), xh.ptr, B, Cin, H * W, label="x.nhwc",
                   spec=dict(kind="nchw_to_nhwc", src=x_in, dst=xh))
         hw = (H, W)
-        h = self.gemm_wo(model.conv_in, self.split3(xh, "conv_in.split"), "conv_in", im2col=(hw, 1, (1, 1), hw))
+        h = self.plane_gemm(model.conv_in, self.split3(xh, "conv_in.split"), "conv_in", im2col=(hw, 1, (1, 1), hw))
         hs = [(h, hw)]
         nres = model.num_resolutions
         for lv in range(nres):
@@ -1464,7 +1447,7 @@ class WeightOnlyBuilder(Builder):
                 conv = st.downsample.conv
                 ohw = (hw[0] // 2, hw[1] // 2)
                 # F.pad (0,1,0,1) then 3x3 stride 2, padding 0 (ddim/models/diffusion.py:67-71)
-                h = self.gemm_wo(conv, self.split3(hs[-1][0], self.key(conv) + ".split"), self.key(conv),
+                h = self.plane_gemm(conv, self.split3(hs[-1][0], self.key(conv) + ".split"), self.key(conv),
                                  im2col=(hw, 2, (0, 0), ohw))
                 hw = ohw
                 hs.append((h, hw))
@@ -1486,9 +1469,9 @@ class WeightOnlyBuilder(Builder):
                 conv = st.upsample.conv
                 a = self.split3(h, self.key(conv) + ".split", upsample=(B, hw[0], hw[1]))
                 hw = (2 * hw[0], 2 * hw[1])
-                h = self.gemm_wo(conv, a, self.key(conv), conv_bhw=(B, hw[0], hw[1]), rows_per_batch=hw[0] * hw[1])
+                h = self.plane_gemm(conv, a, self.key(conv), hw=hw, rows_per_batch=hw[0] * hw[1])
         hn = self.gn_f32(h, model.norm_out, hw[0] * hw[1], True, "norm_out")
-        o = self.gemm_wo(model.conv_out, self.split3(hn, "conv_out.split"), "conv_out", conv_bhw=(B, hw[0], hw[1]),
+        o = self.plane_gemm(model.conv_out, self.split3(hn, "conv_out.split"), "conv_out", hw=hw,
                          rows_per_batch=hw[0] * hw[1])
         out = torch.zeros((B, o.cols, hw[0], hw[1]), dtype=torch.float32, device=self.dev)   # o.cols: out_ch padded to 4
         self.keep.append(out)
@@ -1526,13 +1509,12 @@ class WeightOnlyBuilder(Builder):
             a1 = self.split3(h1, k + ".in_layers.2.split")
         emb_out = self.lin(blk.emb_layers[1], emb, k + ".emb_layers.1", act=1)
         oc = int(conv2.weight.shape[0])
-        cb = (self.B, oh, ow)
         if getattr(blk, "use_scale_shift_norm", False):
-            h = self.gemm_wo(conv1, a1, k + ".in_layers.2", conv_bhw=cb, rows_per_batch=oh * ow)
+            h = self.plane_gemm(conv1, a1, k + ".in_layers.2", hw=(oh, ow), rows_per_batch=oh * ow)
             ss = (emb_out.t, _Offset(emb_out.t, 4 * oc), emb_out.ld)
             h2 = self.gn_f32(h, norm2, oh * ow, True, k + ".out_layers.0", ss=ss, ss_src=(emb_out, oc))
         else:
-            h = self.gemm_wo(conv1, a1, k + ".in_layers.2", conv_bhw=cb, rows_per_batch=oh * ow, rowvec=emb_out)
+            h = self.plane_gemm(conv1, a1, k + ".in_layers.2", hw=(oh, ow), rows_per_batch=oh * ow, rowvec=emb_out)
             h2 = self.gn_f32(h, norm2, oh * ow, True, k + ".out_layers.0")
         skip = blk.skip_connection
         s_ = x_res
@@ -1540,7 +1522,7 @@ class WeightOnlyBuilder(Builder):
             if skip.weight.shape[-1] != 1:
                 raise NotImplementedError("3x3 skip_connection (use_conv=True) is not used by any reference config")
             s_ = self.shortcut(skip, x_res, k + ".skip_connection", split)
-        out = self.gemm_wo(conv2, self.split3(h2, k + ".out_layers.3.split"), k + ".out_layers.3", conv_bhw=cb,
+        out = self.plane_gemm(conv2, self.split3(h2, k + ".out_layers.3.split"), k + ".out_layers.3", hw=(oh, ow),
                            rows_per_batch=oh * ow, residual=s_)
         return out, (oh, ow)
 
@@ -1551,8 +1533,8 @@ class WeightOnlyBuilder(Builder):
         d = inner // heads
         q = self.lin(attn.to_q, xq, label + ".to_q")
         a_kv = self.split3(xkv, label + ".kv.split")
-        kk = self.gemm_wo(attn.to_k, a_kv, label + ".to_k")
-        v = self.gemm_wo(attn.to_v, a_kv, label + ".to_v")
+        kk = self.plane_gemm(attn.to_k, a_kv, label + ".to_k")
+        v = self.plane_gemm(attn.to_v, a_kv, label + ".to_v")
         o = self.attention_fp(q, kk, v, heads=heads, d=d, Tq=Tq, Tk=Tk, q_layout=(0, d), k_layout=(0, d), v_layout=(0, d),
                               scale=float(attn.scale), label=label + ".attn")
         return self.lin(attn.to_out[0], o, label + ".to_out.0", residual=h_res)
@@ -1615,7 +1597,7 @@ class WeightOnlyBuilder(Builder):
             for layer in seq:
                 n = _name(layer)
                 if n == "QuantModule":                       # conv_in
-                    h = self.gemm_wo(layer, self.split3(h, self.key(layer) + ".split"), self.key(layer),
+                    h = self.plane_gemm(layer, self.split3(h, self.key(layer) + ".split"), self.key(layer),
                                      im2col=(hw, 1, (1, 1), hw))
                 elif n in _RES:
                     h, hw = self.wo_resblock(layer, h, emb, hw, split)
@@ -1628,13 +1610,13 @@ class WeightOnlyBuilder(Builder):
                     if _name(op) != "QuantModule":
                         raise NotImplementedError("Downsample without conv")
                     ohw = (hw[0] // 2, hw[1] // 2)
-                    h = self.gemm_wo(op, self.split3(h, self.key(op) + ".split"), self.key(op), im2col=(hw, 2, (1, 1), ohw))
+                    h = self.plane_gemm(op, self.split3(h, self.key(op) + ".split"), self.key(op), im2col=(hw, 2, (1, 1), ohw))
                     hw = ohw
                 elif n == "Upsample":
                     conv = layer.conv
                     a = self.split3(h, self.key(conv) + ".split", upsample=(self.B, hw[0], hw[1]))
                     hw = (2 * hw[0], 2 * hw[1])
-                    h = self.gemm_wo(conv, a, self.key(conv), conv_bhw=(self.B, hw[0], hw[1]), rows_per_batch=hw[0] * hw[1])
+                    h = self.plane_gemm(conv, a, self.key(conv), hw=hw, rows_per_batch=hw[0] * hw[1])
                 else:
                     raise NotImplementedError(f"unhandled layer type {n} at {self.key(layer)}")
             return h, hw
@@ -1653,7 +1635,7 @@ class WeightOnlyBuilder(Builder):
             h, hw = run(blk, h, hw, split)
             self.traces[f"output_blocks.{i}"] = (h, hw)
         hn = self.gn_f32(h, model.out[0], hw[0] * hw[1], True, "out.0")
-        o = self.gemm_wo(model.out[2], self.split3(hn, "out.2.split"), "out.2", conv_bhw=(B, hw[0], hw[1]),
+        o = self.plane_gemm(model.out[2], self.split3(hn, "out.2.split"), "out.2", hw=hw,
                          rows_per_batch=hw[0] * hw[1])
         out = torch.zeros((B, o.cols, hw[0], hw[1]), dtype=torch.float32, device=self.dev)   # o.cols: out channels padded to 4
         self.keep.append(out)
@@ -1712,9 +1694,6 @@ class _WQView:
 def compile_unet(qnn, x_shape, ctx_shape, device, use_cuda_graph=True, cfg_dedup=False):
     """Lower `qnn` (QuantModel) for a fixed input shape; returns a Program.  cfg_dedup: x_shape / ctx_shape describe the
     doubled classifier-free-guidance batch, the program takes x and timesteps of HALF that batch (Builder.cfg_split)."""
-    lib()  # fail loudly if the CUDA library is missing
-    if not torch.cuda.is_available():
-        raise RuntimeError("qdiff_b200: no CUDA device; the engine has no CPU fallback")
     states = {(m.use_weight_quant, m.use_act_quant) for m in qnn.model.modules() if _name(m) == "QuantModule"}
     if states == {(True, True)}:
         b = Builder(qnn, device, x_shape[0])
@@ -1737,11 +1716,4 @@ def compile_unet(qnn, x_shape, ctx_shape, device, use_cuda_graph=True, cfg_dedup
             x_in, t_in, ctx_in, out = b.lower_ddim(model, x_shape)
         else:
             raise NotImplementedError(f"unknown UNet type {_name(model)}")
-    b.flush()
-    check(lib().qd_engine_finalize(b.engine), "qd_engine_finalize")
-    prog = Program(b.engine, b.keep, x_in, t_in, ctx_in, out, b.nops, b.traces, use_cuda_graph, n_static=b.n_static)
-    prog.op_names, prog.op_kinds, prog.op_flops = b.op_names, b.op_kinds, b.op_flops
-    prog.kernel_launches = sum(3 if k == _lib.QD_OP_GROUPNORM else 1 for k in b.op_kinds[b.n_static:])   # until the first run
-    prog.layer_traces = b.layer_traces
-    prog.op_specs = b.op_specs
-    return prog
+    return b.finish(Program, x_in, t_in, ctx_in, out, use_cuda_graph)

@@ -21,7 +21,7 @@ import os
 
 import torch
 
-from . import ops, unet
+from . import graph, ops, unet
 from .quant_layer import QuantModule, UniformAffineQuantizer
 from .quant_model import QuantModel
 
@@ -79,26 +79,31 @@ def export_packed(qnn, path, example_inputs=None):
     layers = {}
     for key, ent in qnn._wcache.items():
         dev, *rest = key
+        if rest[0] == "planes":                  # weight-only operand (graph.WeightOnlyBuilder.plane_weights)
+            _, label, cols, suffix, passes, _ = rest
+            if passes != graph._CODES:           # from fp32 weights: a packed model has none and never runs that state
+                continue
+            # the bfloat16 [N, taps, 3, Cp] tile as the engine reads it, under the layer name of format version 2
+            layers[repr(("wo", label, cols, suffix, ent["taps"] == 9))] = dict(
+                w8=False, N=ent["N"], taps=ent["taps"], w_rows=ent["N"], delta_w=ent["scale"].detach().cpu(),
+                w=ent["tiles"][0][0].detach().cpu(), packed=False, N_real=ent["N_real"], weight_only=True)
+            continue
         name = repr(tuple(rest))
         if ent.get("w8"):
             layers[name] = dict(w8=True)
             continue
         w = ent["w_dev"].detach().cpu()
-        rec = dict(w8=False, N=ent["N"], taps=ent.get("taps", 1), w_rows=ent.get("w_rows", ent["N"]),
-                   delta_w=ent["delta_w"].detach().cpu())
-        if "Cred" in ent:                        # INT8-path operand (quantised activations)
-            rec.update(Cred=ent["Cred"], kdup=ent.get("kdup", 1), wsum=ent["wsum"].detach().cpu(),
-                       perm=None if ent["perm"] is None else ent["perm"].detach().cpu())
-            if ent["w_zero"] is not None:        # already packed (QDIFF_W4_PACKED=1)
-                rec.update(w=w, w_zero=ent["w_zero"].detach().cpu(), packed=True)
+        rec = dict(w8=False, N=ent["N"], taps=ent["taps"], w_rows=ent["w_rows"], delta_w=ent["delta_w"].detach().cpu(),
+                   Cred=ent["Cred"], kdup=ent["kdup"], wsum=ent["wsum"].detach().cpu(),
+                   perm=None if ent["perm"] is None else ent["perm"].detach().cpu())
+        if ent["w_zero"] is not None:            # already packed (QDIFF_W4_PACKED=1)
+            rec.update(w=w, w_zero=ent["w_zero"].detach().cpu(), packed=True)
+        else:
+            pk = ops.pack_int4(w.reshape(w.shape[0], -1))
+            if pk is not None:                   # 4-bit layer: two codes per byte on disk
+                rec.update(w=pk[0], w_zero=pk[1], packed=True, w_shape=tuple(w.shape))
             else:
-                pk = ops.pack_int4(w.reshape(w.shape[0], -1))
-                if pk is not None:               # 4-bit layer: two codes per byte on disk
-                    rec.update(w=pk[0], w_zero=pk[1], packed=True, w_shape=tuple(w.shape))
-                else:
-                    rec.update(w=w, packed=False)
-        else:                                    # weight-only operand: the bfloat16 [N, taps, 3, Cp] tile as the engine reads it
-            rec.update(w=w, packed=False, N_real=ent.get("N_real", ent["N"]), weight_only=True)
+                rec.update(w=w, packed=False)
         layers[name] = rec
     small, act, splits = {}, {}, {}
     for n, p_ in qnn.model.named_parameters():
@@ -166,10 +171,10 @@ def load_packed(path, device="cuda", cuda_graph=True):
     cache = {}
     for name, rec in blob["layers"].items():
         rest = ast.literal_eval(name)                        # a tuple of str / int / bool / None literals
-        if rec.get("weight_only"):
-            key = (idx,) + rest
-            cache[key] = dict(w_dev=rec["w"].to(dev), delta_w=rec["delta_w"].to(dev), N=rec["N"], N_real=rec["N_real"],
-                              taps=rec["taps"])
+        if rec.get("weight_only"):                          # name ("wo", label, cols, suffix, conv): integer codes
+            _, label, cols, suffix, _ = rest
+            cache[(idx, "planes", label, cols, suffix, graph._CODES, (3,))] = dict(
+                tiles=[(rec["w"].to(dev), 3)], scale=rec["delta_w"].to(dev), N=rec["N"], N_real=rec["N_real"], taps=rec["taps"])
             continue
         rest = rest[:-1] + (want_packed,)                    # last key field: packed-in-HBM layout of this run
         key = (idx,) + rest

@@ -387,6 +387,7 @@ K_CHUNK = 256
 
 class TextEncoderBuilder(graph.WeightOnlyBuilder):
     """CLIPTextTransformer.forward as engine ops (fp32 activations, fp32-faithful bfloat16-plane GEMMs)."""
+    precision = 6
 
     def linear(self, lin, x, label, act=0, residual=None):
         """y = x W^T + b (+ residual) as accumulating launches over K_CHUNK-column slices of x (and of W)."""
@@ -395,10 +396,8 @@ class TextEncoderBuilder(graph.WeightOnlyBuilder):
         for c0 in range(0, K, step):
             c1 = min(K, c0 + step)
             a = self.split3(x.view(c0, c1 - c0), f"{label}.split{c0}", act=act)
-            o = self._gemm_fp_weights(lin, a, label if o is None else f"{label}.k{c0}", conv_bhw=None, rowvec=None,
-                                      residual=residual if o is None else None, out=None, rows_per_batch=0,
-                                      cols=(c0, c1) if c1 - c0 < K else None, accumulate_into=o, use_bias=o is None,
-                                      im2col=None)
+            o = self.plane_gemm(lin, a, label if o is None else f"{label}.k{c0}", cols=(c0, c1) if c1 - c0 < K else None,
+                                residual=residual if o is None else None, accumulate_into=o, use_bias=o is None)
         return o
 
     def lower(self, enc):
@@ -433,8 +432,8 @@ class TextEncoderBuilder(graph.WeightOnlyBuilder):
 class TextProgram:
     """One lowered encoder for a fixed batch size: copy the ids into the static buffer, replay (one CUDA graph)."""
 
-    def __init__(self, engine, keep, ids_in, out, nops, use_cuda_graph, B, T, C_):
-        self.engine, self.keep, self.ids_in, self.out, self.nops = engine, keep, ids_in, out, nops
+    def __init__(self, engine, keep, ids_in, out, use_cuda_graph, B, T, C_):
+        self.engine, self.keep, self.ids_in, self.out = engine, keep, ids_in, out
         self.use_cuda_graph, self.shape, self.graph = use_cuda_graph, (B, T, C_), None
 
     def _launch(self):
@@ -464,17 +463,10 @@ class TextProgram:
 
 
 def compile_text_encoder(enc, batch, device, use_cuda_graph=True):
-    lib()       # fail loudly if the CUDA library is missing
-    if not torch.cuda.is_available():
-        raise RuntimeError("qdiff_b200: no CUDA device; the engine has no CPU fallback")
     b = TextEncoderBuilder(enc, device, batch)
     with torch.no_grad():
         ids_in, z = b.lower(enc)
-    b.flush()
-    check(lib().qd_engine_finalize(b.engine), "qd_engine_finalize")
-    prog = TextProgram(b.engine, b.keep, ids_in, z, b.nops, use_cuda_graph, batch, enc.max_length, enc.width)
-    prog.op_names, prog.op_kinds, prog.traces = b.op_names, b.op_kinds, b.traces
-    return prog
+    return b.finish(TextProgram, ids_in, z, use_cuda_graph, batch, enc.max_length, enc.width)
 
 
 def build_text_encoder(state_dict, tokenizer_dir=None, version=DEFAULT_VERSION, heads=None, **kw):

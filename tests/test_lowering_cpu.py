@@ -1,20 +1,32 @@
 """Host-side graph builders without a GPU: tools/dryrun_lowering.py replaces the C library by a recorder (every entry point
-succeeds, tensors on the CPU) and lowers the first stage, the weight-only / full-precision UNet states and the INT8 DDIM
-family.  Run in a subprocess (it patches module globals).  Nothing is computed: this pins the STRUCTURE of the recorded
-programs - op counts, the copy-free decoder concat - so a lowering mistake shows up in the CPU suite already."""
+succeeds, tensors on the CPU) and lowers the first stage, the weight-only / full-precision UNet states, the INT8 DDIM
+family and the text encoder.  Run in a subprocess (it patches module globals).  Nothing is computed: this pins the
+STRUCTURE of the recorded programs - op counts, the copy-free decoder concat, and a digest of every op's descriptor and
+of the buffers it reads (tests/golden/lowering_digests.json) - so a lowering mistake shows up in the CPU suite already."""
+import ast
+import json
 import os
 import re
 import subprocess
 import sys
 
+import pytest
+
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
-def test_lowerings_dry_run():
-    r = subprocess.run([sys.executable, os.path.join(ROOT, "tools", "dryrun_lowering.py")], capture_output=True, text=True,
-                       timeout=600, cwd=ROOT)
+@pytest.fixture(scope="module")
+def dry_run(tmp_path_factory):
+    path = tmp_path_factory.mktemp("lowering") / "digests.json"
+    r = subprocess.run([sys.executable, os.path.join(ROOT, "tools", "dryrun_lowering.py"), "--digests", str(path)],
+                       capture_output=True, text=True, timeout=900, cwd=ROOT)
     assert r.returncode == 0, r.stdout[-1500:] + r.stderr[-3000:]
-    out = r.stdout
+    with open(path) as f:
+        return r.stdout, json.load(f)
+
+
+def test_lowerings_dry_run(dry_run):
+    out = dry_run[0]
     ops = {m.group(1).strip(): int(m.group(2)) for m in re.finditer(r"^(.*?): (\d+) ops", out, re.M)}
     # first stage: one conv = 1 / 2 / 3 accumulating launches with the precision; the VQ first stage adds the codebook lookup
     assert ops["first stage sd_v1 precision 1"] < ops["first stage sd_v1 precision 3"] < ops["first stage sd_v1 precision 6"]
@@ -26,6 +38,44 @@ def test_lowerings_dry_run():
     m = re.search(r"QDIFF_DDIM_CAT=inplace: (\d+) ops, (\d+) copy2d", out)
     c = re.search(r"QDIFF_DDIM_CAT=copy: (\d+) ops, (\d+) copy2d", out)
     assert m and c and int(m.group(2)) == 0 and int(c.group(2)) == 8 and int(c.group(1)) - int(m.group(1)) == 8
+
+
+def test_op_streams_match_golden_digests(dry_run):
+    """Every dry-run program records exactly the op stream of the golden file: same ops in engine order, same descriptor
+    fields, same buffer layout and contents, same op_flops total."""
+    with open(os.path.join(ROOT, "tests", "golden", "lowering_digests.json")) as f:
+        gold = json.load(f)
+    got = dry_run[1]
+    assert sorted(got) == sorted(gold)
+    bad = {k: (got[k], gold[k]) for k in gold if got[k] != gold[k]}
+    assert not bad, "\n".join(f"{k}: got {a}, golden {b}" for k, (a, b) in bad.items())
+
+
+def test_export_packed_skips_fp32_weight_entries(monkeypatch, tmp_path):
+    """A model that ran in the weight-only AND the full-precision state caches operands of both kinds; its engine-native
+    checkpoint holds the integer-code ones only (a packed model has no fp32 weights, so it never runs that state), one per
+    layer under the layer names of the file format."""
+    import torch
+    from qdiff_b200 import graph, packed
+    from tests.test_oracle_golden import load_case
+    from tests.test_unet_gpu import build_qnn
+    from tools.dryrun_lowering import install_fake_lib
+    install_fake_lib(monkeypatch.setattr)
+    cpu = torch.device("cpu")
+    g = load_case("ddim_w8_weightonly")
+    qnn = build_qnn(g, cpu)
+    for state in ((True, False), (False, False)):
+        qnn.set_quant_state(*state)
+        with torch.no_grad():
+            graph.WeightOnlyBuilder(qnn, cpu, g["x"].shape[0]).lower_ddim(qnn.model, tuple(g["x"].shape))
+    packed.export_packed(qnn, str(tmp_path / "model.qdpk"))
+    layers = torch.load(tmp_path / "model.qdpk", weights_only=False)["layers"]
+    modules = {k for k, m in qnn.model.named_modules() if type(m).__name__ == "QuantModule"}
+    names = [ast.literal_eval(n) for n in layers]
+    assert sorted(n[1] for n in names) == sorted(modules)
+    for n, rec in zip(names, layers.values()):
+        assert n[0] == "wo" and rec["weight_only"] and rec["w"].dtype == torch.bfloat16
+        assert rec["w"].shape[0] == rec["N"] == rec["delta_w"].numel() >= rec["N_real"]
 
 
 def test_implicit_conv_rule():
