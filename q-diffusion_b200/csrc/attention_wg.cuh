@@ -6,10 +6,10 @@
 //     wgmma width (the extra rows: the all-ones row, then zeros);
 //   * K, V^T and the zq*rowsum(k) slice staged by TMA / bulk copies through an ATW_STAGES-deep mbarrier ring (one load
 //     per (pass, key tile); pass 0 needs no V^T).  The consumer warp that releases a stage last refills it.
-// Two consumer warpgroups, 64 query rows each, running the loads L = 0 .. 2*ntiles-1 of both passes in one sequence;
-// for d <= 40 two CTAs share an SM (MINB = 2, <= 128 registers).  On fp16 operands the fp32 scores are used as they are
-// (exact integers), with no conversion to int32.  The per-warp accumulator fragment of wgmma m64nN is the m16n8 fragment
-// of mma.sync repeated over N / 8 column tiles, and the register A operand has the m16n8k32 layout, so the softmax code
+// Two consumer warpgroups, 64 query rows each, running the loads L = 0 .. 2*ntiles-1 in order, one loop per pass;
+// for d <= 40 two CTAs share an SM (MINB = 2, <= 128 registers).  The softmax works on fp32 scores: the fp16 operands'
+// accumulators as they are (exact integers), and the 8-bit codes' int32 sums converted without I2F.  The per-warp
+// accumulator fragment of wgmma m64nN is the m16n8 fragment of mma.sync repeated over N / 8 column tiles, and the register A operand has the m16n8k32 layout, so the softmax code
 // below is qattention_kernel's, operating on the same registers.  V^T keeps its 16-key byte permutation
 // (att_vt_perm): with it, the P fragments built from the S accumulators are the A operand without shuffles.
 #pragma once
@@ -222,10 +222,16 @@ qattention_wg_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_const
   constexpr int NV = atw_nv(DV);
   constexpr int NKC = DQ / 32;      // 32-byte k-steps of QK^T
   constexpr int NDT = DV / 8 + 1;   // n8 tiles of the output + the row-sum tile
-  constexpr bool MAGIC = DV <= 64;  // |S| <= 255*255*d < 2^22
   constexpr int RB = F16 ? 2 * DV : DV;   // bytes of one head's Q / K row
   static_assert(!F16 || DV <= 64, "fp16 Q / K operands: d <= 64 keeps |S| below 2^22");
-  using SV = att_score_t<F16>;      // score: int32, or the exact fp32 accumulator
+  static_assert(DV <= 96, "8-bit codes: the raw scores must stay below 2^23 (unsigned) / 2^22 (signed)");
+  // Accumulator of S = Q K^T: the exact fp32 score on fp16 operands; the raw int32 sum on 8-bit codes, made fp32 without
+  // I2F (which shares the quarter-rate pipe with ex2): the bits of MB + raw are the float MB + raw, exact for unsigned
+  // codes (MB = 2^23, 0 <= raw <= 255^2 * 96 < 2^23) and signed ones (MB = 1.5 * 2^23, |raw| <= 128^2 * 96 < 2^22).
+  // zq * rowsum(k) goes through the same add (attention_wg_eligible keeps it in that range), and the difference of two
+  // floats of [2^22, 2^24) with unit spacing is the exact score.
+  using SV = std::conditional_t<F16, float, uint32_t>;
+  constexpr uint32_t MB = QK_SIGNED ? 0x4B400000u : 0x4B000000u;
   extern __shared__ uint8_t atw_raw[];
   uint8_t* smem = atw_raw + (((smem_u32(atw_raw) + 1023u) & ~1023u) - smem_u32(atw_raw));
   const AtwSmem lay = atw_smem(P, NV);
@@ -295,12 +301,8 @@ qattention_wg_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_const
   if constexpr (!QRELOAD) load_q();
   const float c = p.sim_scale * 1.4426950408889634f;
   const bool ragged = (p.Tk % ATT_BN) != 0;
-  SV mi0 = att_lowest(SV{}), mi1 = att_lowest(SV{});
+  float mi0 = -INFINITY, mi1 = -INFINITY;
   float l0 = 0.f, l1 = 0.f;
-  float off0 = 0.f, off1 = 0.f;
-  uint32_t olo[NV / 2], ohi[SM16 ? NV / 2 : 1];     // zeroed by the first PV (scale_d = 0)
-  const float pmax = (float)p.p_qmax;
-  const QuantK oqk = make_quantk(p.oq);
 
   // S(L) = Q K^T for this warpgroup, 64 x 64, once load L has landed; this warp's 16 rows land in s[nt][0..3]
   // (m16n8 fragments)
@@ -313,10 +315,41 @@ qattention_wg_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_const
 #pragma unroll
     for (int kc = 0; kc < NKC; ++kc) {
       if constexpr (F16) wgmma_ra_f16_n64(&s[0][0], qf[kc], dK + (uint64_t)(2 * kc), kc ? 1u : 0u);
-      else if constexpr (QK_SIGNED) wgmma_ra_s8s8_n64(reinterpret_cast<uint32_t*>(&s[0][0]), qf[kc], dK + (uint64_t)(2 * kc), kc ? 1u : 0u);
-      else wgmma_ra_u8u8_n64(reinterpret_cast<uint32_t*>(&s[0][0]), qf[kc], dK + (uint64_t)(2 * kc), kc ? 1u : 0u);
+      else if constexpr (QK_SIGNED) wgmma_ra_s8s8_n64(&s[0][0], qf[kc], dK + (uint64_t)(2 * kc), kc ? 1u : 0u);
+      else wgmma_ra_u8u8_n64(&s[0][0], qf[kc], dK + (uint64_t)(2 * kc), kc ? 1u : 0u);
     }
     wgmma_commit();
+  };
+  // After the wait that retired S(L): the fp32 scores, keys beyond Tk at -inf (no share of the row maximum, the row sum
+  // or the P codes, whatever the codes are).
+  auto scores = [&](SV (&s)[8][4], float (&f)[8][4], int L) {
+    wgmma_fence_regs(reinterpret_cast<SV (&)[32]>(s));
+    const int tile = L % ntiles, st = L % ATW_STAGES;
+    if constexpr (F16) {
+#pragma unroll
+      for (int i = 0; i < 32; ++i) f[i >> 2][i & 3] = s[i >> 2][i & 3];
+    } else {
+      const uint32_t* sZrk = reinterpret_cast<const uint32_t*>(smem + lay.z_off + st * ATT_BN * 4);
+#pragma unroll
+      for (int nt = 0; nt < 8; ++nt) {
+        float z0 = __uint_as_float(MB), z1 = z0;
+        if (has_zq) {
+          const uint2 z = *reinterpret_cast<const uint2*>(sZrk + 8 * nt + 2 * t);
+          z0 = __uint_as_float(z.x + MB);
+          z1 = __uint_as_float(z.y + MB);
+        }
+        f[nt][0] = __uint_as_float(s[nt][0] + MB) - z0; f[nt][1] = __uint_as_float(s[nt][1] + MB) - z1;
+        f[nt][2] = __uint_as_float(s[nt][2] + MB) - z0; f[nt][3] = __uint_as_float(s[nt][3] + MB) - z1;
+      }
+    }
+    if (ragged && tile == ntiles - 1) {
+#pragma unroll
+      for (int nt = 0; nt < 8; ++nt) {
+        const int j = tile * ATT_BN + 8 * nt + 2 * t;
+        if (j >= p.Tk) { f[nt][0] = -INFINITY; f[nt][2] = -INFINITY; }
+        if (j + 1 >= p.Tk) { f[nt][1] = -INFINITY; f[nt][3] = -INFINITY; }
+      }
+    }
   };
 
   // Release load R; the last of the 8 warps to do so refills the stage, so no warp waits for another.
@@ -333,106 +366,94 @@ qattention_wg_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_const
     }
   };
 
-  // Softmax of the completed scores S(L) (edited in place) and, in pass 1, PV(L) issued and committed.
-  auto softmax_pv = [&](SV (&sacc)[8][4], int L) {
-    const int pass = L >= ntiles ? 1 : 0, tile = L - pass * ntiles, st = L % ATW_STAGES;
-    const int j0 = tile * ATT_BN;
-    if (L == ntiles) {
-      l0 += __shfl_xor_sync(0xffffffffu, l0, 1);
-      l0 += __shfl_xor_sync(0xffffffffu, l0, 2);
-      l1 += __shfl_xor_sync(0xffffffffu, l1, 1);
-      l1 += __shfl_xor_sync(0xffffffffu, l1, 2);
-      off0 = -(float)mi0 * c + log2f(1.0f / (l0 * p.delta_w));
-      off1 = -(float)mi1 * c + log2f(1.0f / (l1 * p.delta_w));
-    }
-    const int* sZrk = reinterpret_cast<const int*>(smem + lay.z_off + st * ATT_BN * 4);
-    if (has_zq) {
-#pragma unroll
-      for (int nt = 0; nt < 8; ++nt) {
-        const int2 z = *reinterpret_cast<const int2*>(sZrk + 8 * nt + 2 * t);
-        sacc[nt][0] -= z.x; sacc[nt][1] -= z.y; sacc[nt][2] -= z.x; sacc[nt][3] -= z.y;
-      }
-    }
-    if (ragged && tile == ntiles - 1) {
-      const SV mask = att_mask<MAGIC>(SV{});
-#pragma unroll
-      for (int nt = 0; nt < 8; ++nt) {
-        const int j = j0 + 8 * nt + 2 * t;
-        if (j >= p.Tk) { sacc[nt][0] = mask; sacc[nt][2] = mask; }
-        if (j + 1 >= p.Tk) { sacc[nt][1] = mask; sacc[nt][3] = mask; }
-      }
-    }
-    if (pass == 0) {
-      SV tm0 = sacc[0][0], tm1 = sacc[0][2];
-#pragma unroll
-      for (int nt = 0; nt < 8; ++nt) {
-        tm0 = att_smax(tm0, att_smax(sacc[nt][0], sacc[nt][1]));
-        tm1 = att_smax(tm1, att_smax(sacc[nt][2], sacc[nt][3]));
-      }
-      tm0 = att_smax(tm0, __shfl_xor_sync(0xffffffffu, tm0, 1));
-      tm0 = att_smax(tm0, __shfl_xor_sync(0xffffffffu, tm0, 2));
-      tm1 = att_smax(tm1, __shfl_xor_sync(0xffffffffu, tm1, 1));
-      tm1 = att_smax(tm1, __shfl_xor_sync(0xffffffffu, tm1, 2));
-      if (tm0 > mi0) { l0 *= (mi0 == att_lowest(SV{})) ? 0.f : ex2_approx((float)(mi0 - tm0) * c); mi0 = tm0; }
-      if (tm1 > mi1) { l1 *= (mi1 == att_lowest(SV{})) ? 0.f : ex2_approx((float)(mi1 - tm1) * c); mi1 = tm1; }
-      const float b0 = -(float)mi0 * c, b1 = -(float)mi1 * c;
-      float a0 = 0.f, a1 = 0.f;
-#pragma unroll
-      for (int nt = 0; nt < 8; ++nt) {
-        a0 += ex2_approx(fmaf(att_s2f<MAGIC>(sacc[nt][0]), c, b0)) + ex2_approx(fmaf(att_s2f<MAGIC>(sacc[nt][1]), c, b0));
-        a1 += ex2_approx(fmaf(att_s2f<MAGIC>(sacc[nt][2]), c, b1)) + ex2_approx(fmaf(att_s2f<MAGIC>(sacc[nt][3]), c, b1));
-      }
-      l0 += a0;
-      l1 += a1;
-    } else {
-      // ---- P codes packed straight into A fragments (byte planes), then O += P V on the warpgroup, left in flight
-      const uint64_t dV = atw_desc(smem_u32(smem + ATW_STAGES * lay.k_bytes + st * lay.v_bytes), ATT_BN);
-      uint32_t plo[2][4], phi[2][4];
-#pragma unroll
-      for (int kc = 0; kc < 2; ++kc) {
-#pragma unroll
-        for (int half = 0; half < 2; ++half) {
-          const int ntA = 4 * kc + 2 * half, ntB = ntA + 1;
-          uint32_t cd[8];
-          const SV sv[8] = {sacc[ntA][0], sacc[ntA][1], sacc[ntB][0], sacc[ntB][1],
-                            sacc[ntA][2], sacc[ntA][3], sacc[ntB][2], sacc[ntB][3]};
-#pragma unroll
-          for (int e = 0; e < 8; ++e) {
-            const float pr = ex2_approx(fmaf(att_s2f<MAGIC>(sv[e]), c, e < 4 ? off0 : off1));
-            cd[e] = __float_as_uint(fminf(pr, pmax) + 12582912.0f);
-          }
-          plo[kc][2 * half] = __byte_perm(__byte_perm(cd[0], cd[1], 0x0040), __byte_perm(cd[2], cd[3], 0x0040), 0x5410);
-          plo[kc][2 * half + 1] = __byte_perm(__byte_perm(cd[4], cd[5], 0x0040), __byte_perm(cd[6], cd[7], 0x0040), 0x5410);
-          if constexpr (SM16) {
-            phi[kc][2 * half] = __byte_perm(__byte_perm(cd[0], cd[1], 0x0051), __byte_perm(cd[2], cd[3], 0x0051), 0x5410);
-            phi[kc][2 * half + 1] = __byte_perm(__byte_perm(cd[4], cd[5], 0x0051), __byte_perm(cd[6], cd[7], 0x0051), 0x5410);
-          }
-        }
-      }
-      wgmma_fence();
-#pragma unroll
-      for (int kc = 0; kc < 2; ++kc) {
-        const uint32_t acc = (kc || L > ntiles) ? 1u : 0u;
-        atw_pv<NV, V_SIGNED>(olo, plo[kc], dV + (uint64_t)(2 * kc), acc);
-        if constexpr (SM16) atw_pv<NV, V_SIGNED>(ohi, phi[kc], dV + (uint64_t)(2 * kc), acc);
-      }
-      wgmma_commit();
-    }
-  };
-
-  // One S register set, every wgmma retired before the next load: few enough registers that, for d <= 40, two CTAs
-  // share an SM and their warps hide each other's latencies (measured: faster than overlapping S(L+1) and PV(L) with
-  // the softmax inside one CTA, which needs a second S set; DESIGN §6).
-  for (int L = 0; L < nloads; ++L) {
+  // One S register set per warp and every wgmma retired before the next is issued: for d <= 40 that fits 128 registers
+  // (two CTAs per SM, whose warps hide each other's latencies) without spills or wgmma serialisation.  Overlapping
+  // S(L+1) with the softmax of S(L) needs a second S set (pass 0) or P and S live together (pass 1); ptxas of CUDA 12.9
+  // then spills or serialises the wgmmas at that register cap (DESIGN §6).
+  // ---- pass 0: row maxima and sums.  The O accumulators are not live yet.  Load L (K and the zq * rowsum(k) slice) is
+  // released as soon as its scores are read, before the exp2 work.
+  for (int L = 0; L < ntiles; ++L) {
     SV sacc[8][4];
     issue_s(sacc, L);
     wgmma_wait<0>();
+    float f[8][4];
+    scores(sacc, f, L);
+    release(L);
+    float tm0 = f[0][0], tm1 = f[0][2];
 #pragma unroll
-    for (int i = 0; i < 32; ++i) {
-      if constexpr (F16) asm volatile("" : "+f"(sacc[i >> 2][i & 3])::"memory");
-      else asm volatile("" : "+r"(sacc[i >> 2][i & 3])::"memory");
+    for (int nt = 0; nt < 8; ++nt) {
+      tm0 = fmaxf(tm0, fmaxf(f[nt][0], f[nt][1]));
+      tm1 = fmaxf(tm1, fmaxf(f[nt][2], f[nt][3]));
     }
-    softmax_pv(sacc, L);
+    tm0 = fmaxf(tm0, __shfl_xor_sync(0xffffffffu, tm0, 1));
+    tm0 = fmaxf(tm0, __shfl_xor_sync(0xffffffffu, tm0, 2));
+    tm1 = fmaxf(tm1, __shfl_xor_sync(0xffffffffu, tm1, 1));
+    tm1 = fmaxf(tm1, __shfl_xor_sync(0xffffffffu, tm1, 2));
+    if (tm0 > mi0) { l0 *= (mi0 == -INFINITY) ? 0.f : ex2_approx((mi0 - tm0) * c); mi0 = tm0; }
+    if (tm1 > mi1) { l1 *= (mi1 == -INFINITY) ? 0.f : ex2_approx((mi1 - tm1) * c); mi1 = tm1; }
+    const float b0 = -mi0 * c, b1 = -mi1 * c;
+    float a0 = 0.f, a1 = 0.f;
+#pragma unroll
+    for (int nt = 0; nt < 8; ++nt) {
+      a0 += ex2_approx(fmaf(f[nt][0], c, b0)) + ex2_approx(fmaf(f[nt][1], c, b0));
+      a1 += ex2_approx(fmaf(f[nt][2], c, b1)) + ex2_approx(fmaf(f[nt][3], c, b1));
+    }
+    l0 += a0;
+    l1 += a1;
+  }
+
+  // ---- pass 1: P codes packed straight into A fragments (byte planes), then O += P V on the warpgroup
+  l0 += __shfl_xor_sync(0xffffffffu, l0, 1);
+  l0 += __shfl_xor_sync(0xffffffffu, l0, 2);
+  l1 += __shfl_xor_sync(0xffffffffu, l1, 1);
+  l1 += __shfl_xor_sync(0xffffffffu, l1, 2);
+  const float off0 = -mi0 * c + log2f(1.0f / (l0 * p.delta_w));
+  const float off1 = -mi1 * c + log2f(1.0f / (l1 * p.delta_w));
+  const float pmax = (float)p.p_qmax;
+  const QuantK oqk = make_quantk(p.oq);
+  // code words of S(L): 1.5 * 2^23 + round(min(p, qmax)), the code in the low 16 bits
+  auto codes = [&](SV (&s)[8][4], uint32_t (&cw)[8][4], int L) {
+    float f[8][4];
+    scores(s, f, L);
+#pragma unroll
+    for (int i = 0; i < 32; ++i)
+      cw[i >> 2][i & 3] = __float_as_uint(fminf(ex2_approx(fmaf(f[i >> 2][i & 3], c, (i & 2) ? off1 : off0)), pmax) + 12582912.0f);
+  };
+  // P codes as A fragments (byte planes) of m64nNk32: k-chunk kc holds key tiles 4kc .. 4kc+3
+  uint32_t plo[2][4], phi[2][4];
+  auto pack = [&](const uint32_t (&cw)[8][4]) {
+#pragma unroll
+    for (int kc = 0; kc < 2; ++kc) {
+#pragma unroll
+      for (int half = 0; half < 2; ++half) {
+        const int ntA = 4 * kc + 2 * half, ntB = ntA + 1;
+        const uint32_t cd[8] = {cw[ntA][0], cw[ntA][1], cw[ntB][0], cw[ntB][1], cw[ntA][2], cw[ntA][3], cw[ntB][2], cw[ntB][3]};
+        plo[kc][2 * half] = __byte_perm(__byte_perm(cd[0], cd[1], 0x0040), __byte_perm(cd[2], cd[3], 0x0040), 0x5410);
+        plo[kc][2 * half + 1] = __byte_perm(__byte_perm(cd[4], cd[5], 0x0040), __byte_perm(cd[6], cd[7], 0x0040), 0x5410);
+        if constexpr (SM16) {
+          phi[kc][2 * half] = __byte_perm(__byte_perm(cd[0], cd[1], 0x0051), __byte_perm(cd[2], cd[3], 0x0051), 0x5410);
+          phi[kc][2 * half + 1] = __byte_perm(__byte_perm(cd[4], cd[5], 0x0051), __byte_perm(cd[6], cd[7], 0x0051), 0x5410);
+        }
+      }
+    }
+  };
+  uint32_t olo[NV / 2], ohi[SM16 ? NV / 2 : 1];     // zeroed by the first PV (scale_d = 0)
+  for (int L = ntiles; L < nloads; ++L) {
+    SV sacc[8][4];
+    uint32_t cw[8][4];
+    issue_s(sacc, L);
+    wgmma_wait<0>();
+    codes(sacc, cw, L);
+    pack(cw);
+    const uint64_t dV = atw_desc(smem_u32(smem + ATW_STAGES * lay.k_bytes + (L % ATW_STAGES) * lay.v_bytes), ATT_BN);
+    wgmma_fence();
+#pragma unroll
+    for (int kc = 0; kc < 2; ++kc) {
+      const uint32_t acc = (kc || L > ntiles) ? 1u : 0u;
+      atw_pv<NV, V_SIGNED>(olo, plo[kc], dV + (uint64_t)(2 * kc), acc);
+      if constexpr (SM16) atw_pv<NV, V_SIGNED>(ohi, phi[kc], dV + (uint64_t)(2 * kc), acc);
+    }
+    wgmma_commit();
     wgmma_wait<0>();
     release(L);
   }

@@ -853,6 +853,8 @@ bool attention_wg_eligible(const qd_attention_desc& d) {
   if (d.q_off != 0 || d.k_off != 0 || (d.ld_k & 15) || (((uintptr_t)d.k) & 15) || (((uintptr_t)d.vt) & 15)) return false;
   if (d.v_off != 0 || d.head_stride_v != d.d || d.v_batch_stride != (long long)d.heads * d.d * d.ld_vt) return false;
   if (d.zq != 0 && !d.qk_f16 && !d.ws) return false;
+  // 8-bit codes: the kernel converts zq * rowsum(k) to fp32 by a magic-number add, exact for zero points of the code range
+  if (!d.qk_f16 && (d.zq > 255 || d.zq < (d.q_signed ? -255 : 0))) return false;
   return true;
 }
 
