@@ -12,6 +12,9 @@ QuantModel(model, weight_quant_params, act_quant_params, sm_abit=8) wraps a UNet
 in place exactly like the reference (layers -> QuantModule, blocks -> Quant*Block) so state-dict
 keys match `ckpt.pth`; `forward(x, timesteps, context)` lowers the tree once per input shape to an
 engine program (qdiff_b200/graph.py) and replays it on the current CUDA stream.
+
+Programs and the folded weights they share are cached on the model.  load_state_dict and resume_cali_model drop both;
+after changing weights or quantizer parameters any other way (for example `.data` writes) call invalidate().
 """
 import torch
 import torch.nn as nn
@@ -88,8 +91,16 @@ class QuantModel(nn.Module):
                 m.checkpoint = grad_ckpt
 
     # ---- the hot path
+    def load_state_dict(self, state_dict, strict=True, **kw):
+        """nn.Module.load_state_dict, then invalidate(): the next call folds the loaded weights."""
+        res = super().load_state_dict(state_dict, strict=strict, **kw)
+        self.invalidate()
+        return res
+
     def invalidate(self):
-        """Drop compiled engine programs AND the folded weights (call after changing quantizer parameters or weights)."""
+        """Drop compiled engine programs AND the folded weights.  load_state_dict and resume_cali_model call it; any other
+        change of weights or quantizer parameters (`.data` writes, in-place edits, new quantizer objects) needs an explicit
+        call, or the next forward runs the weights folded before the change."""
         self._programs = {}
         self._wcache = {}
         self._int8_state = None

@@ -34,7 +34,9 @@ def _set_act(q, delta, zero_point):
 
 
 def load_cali_state(qnn, ckpt, quant_act=False):
-    """Materialise quantizer parameters from a ckpt-format dict.  Returns the number of tensors consumed."""
+    """Materialise quantizer parameters from a ckpt-format dict.  Returns the number of tensors consumed.  Drops the
+    model's compiled programs and folded weights (QuantModel.invalidate): a model that already ran would otherwise keep
+    the previous checkpoint's integer weights and steps next to this one's biases and quantizers."""
     mods = dict(qnn.named_modules())
     used = set()
 
@@ -75,6 +77,7 @@ def load_cali_state(qnn, ckpt, quant_act=False):
             with torch.no_grad():
                 m.weight.copy_(take(name + ".weight"))
                 m.bias.copy_(take(name + ".bias"))
+    qnn.invalidate()
     missing = [k for k in ckpt if k not in used and (quant_act or "act" not in k)]
     if missing:
         raise KeyError(f"checkpoint keys not consumed by the model: {missing[:8]} (+{max(0, len(missing) - 8)} more)")
