@@ -144,6 +144,8 @@ _DDIM_ATTN = ("AttnBlock", "QuantAttnBlock")
 
 
 class Builder:
+    concat_in_place = True   # the two producers of a decoder concat write their halves of one buffer (no copies)
+
     def __init__(self, qnn, device, batch):
         self.qnn, self.dev, self.B = qnn, device, batch
         self.names = {id(m): n for n, m in qnn.named_modules()}
@@ -618,11 +620,26 @@ class Builder:
             self.layer_traces[label] = o
         return oq_act if out_q is not None else o
 
-    def qlinear(self, qm, x_f32, label, act=0, **kw):
+    def linear_f32(self, qm, x_f32, label, act=0, **kw):
         """fp32 activation -> this module's input quantizer -> GEMM (QuantModule.forward, quant_layer.py:248-279)."""
         cols = x_f32.cols // 2 if act == 2 else x_f32.cols
         a = self.quantize(x_f32, qm.act_quantizer, label + ".q", act=act, out_cols=cols)
         return self.gemm(qm, a, label, **kw)
+
+    def conv_f32(self, qm, x, hw, label, stride=1, pad_tl=(1, 1), upsample=False, out=None):
+        """3x3 conv of an fp32 map through the explicit patch gather (conv_in, stride-2 downsampling), or after a nearest
+        2x upsample fused into the quantizer.  Returns (output, its (H, W))."""
+        a = self.quantize(x, qm.act_quantizer, label + ".q", upsample=(self.B, hw[0], hw[1]) if upsample else None)
+        if upsample:
+            hw = (2 * hw[0], 2 * hw[1])
+            return self.conv3x3_s1(qm, a, hw, label, out=out), hw
+        ohw = (hw[0] // stride, hw[1] // stride)
+        return self.conv_im2col(qm, a, hw, label, stride, pad_tl, ohw, (9 * x.cols + 31) // 32 * 32, out=out), ohw
+
+    def out_head(self, norm, conv, h, hw):
+        """GroupNorm + SiLU (quantising for the conv) + 3x3 conv: the UNet's output layers."""
+        (a,), _ = self.groupnorm(h, norm, hw[0] * hw[1], [conv.act_quantizer], True, self.key(norm))
+        return self.conv3x3_s1(conv, a, hw, self.key(conv))
 
     @staticmethod
     def implicit_conv_ok(H, W):
@@ -772,7 +789,7 @@ class Builder:
                 x_res = self.new_f32(self.B * oh * ow, x.cols)
                 self.misc(_lib.QD_OP_AVGPOOL2X, x.ptr, x_res.ptr, self.B, H, W, x.cols, label=k + ".x_upd",
                           spec=dict(kind="avgpool2x", src=x, dst=x_res, B=self.B, H=H, W=W))
-        emb_out = self.qlinear(lin, emb, k + ".emb_layers.1", act=1)
+        emb_out = self.linear_f32(lin, emb, k + ".emb_layers.1", act=1)
         oc = conv2.weight.shape[0]
         if getattr(blk, "use_scale_shift_norm", False):
             h = self.conv3x3_s1(conv1, a1, (oh, ow), k + ".in_layers.2")
@@ -796,7 +813,7 @@ class Builder:
             elif a_skip is not None:
                 s = self.gemm(skip, a_skip, k + ".skip_connection")
             else:
-                s = self.qlinear(skip, x_res, k + ".skip_connection")
+                s = self.linear_f32(skip, x_res, k + ".skip_connection")
         else:
             s = x_res
         out = self.conv3x3_s1(conv2, a2, (oh, ow), k + ".out_layers.3", residual=s, out=out)
@@ -888,30 +905,47 @@ class Builder:
                            consumer=blk.proj_out)
         return self.gemm(blk.proj_out, o, k + ".proj_out", residual=x, out=out)
 
-    def lower_ldm(self, model, x_shape, ctx_shape, cfg_dedup=False):
-        B, Cin, H, W = x_shape
-        if cfg_dedup:
-            if B % 2 or ctx_shape is None or ctx_shape[0] != B:
-                raise ValueError("cfg_dedup needs an even batch [uncond; cond] with one context row per sample")
-            self.B, self.prefix = B // 2, True        # record the guidance-invariant prefix for the first half only
-            B = self.B
-        x_in = torch.zeros((B,) + tuple(x_shape[1:]), dtype=torch.float32, device=self.dev)
+    def _prologue(self, x_shape, ctx_shape, ch, mode, dense0, dense1):
+        """The input buffers (x and t of self.B rows: half the batch inside the guidance prefix), the timestep embedding
+        (mode 0: LDM, 1: DDIM) through the two time-embedding linears, and x in NHWC."""
+        B, Cin, H, W = (self.B,) + tuple(x_shape[1:])
+        x_in = torch.zeros((B, Cin, H, W), dtype=torch.float32, device=self.dev)
         t_in = torch.zeros(B, dtype=torch.float32, device=self.dev)
         ctx_in = torch.zeros(ctx_shape, dtype=torch.float32, device=self.dev) if ctx_shape is not None else None
         self.keep += [x_in, t_in] + ([ctx_in] if ctx_in is not None else [])
-        mc = model.model_channels
-        temb = self.new_f32(B, mc)
-        self.misc(_lib.QD_OP_TIMESTEP_EMB, t_in.data_ptr(), temb.ptr, B, mc, 0, label="timestep_embedding",
-                  aux=ops.timestep_freqs(mc, 0).to(self.dev), spec=dict(kind="timestep_emb", t=t_in, dst=temb, mode=0))
-        e = self.qlinear(model.time_embed[0], temb, "time_embed.0")
-        emb = self.qlinear(model.time_embed[2], e, "time_embed.2", act=1)
-        ctx = None
-        if ctx_in is not None:
-            ctx = (Act(ctx_in, ctx_shape[0] * ctx_shape[1], ctx_shape[2]), ctx_shape[1])
+        temb = self.new_f32(B, ch)
+        self.misc(_lib.QD_OP_TIMESTEP_EMB, t_in.data_ptr(), temb.ptr, B, ch, mode, label="timestep_embedding",
+                  aux=ops.timestep_freqs(ch, mode).to(self.dev), spec=dict(kind="timestep_emb", t=t_in, dst=temb, mode=mode))
+        e = self.linear_f32(dense0, temb, self.key(dense0))
+        emb = self.linear_f32(dense1, e, self.key(dense1), act=1)
         xh = self.new_f32(B * H * W, Cin)
         self.misc(_lib.QD_OP_NCHW_TO_NHWC, x_in.data_ptr(), xh.ptr, B, Cin, H * W, label="x.nhwc",
                   spec=dict(kind="nchw_to_nhwc", src=x_in, dst=xh))
-        h, hw = xh, (H, W)
+        return x_in, t_in, ctx_in, emb, xh
+
+    def _epilogue(self, norm, conv, h, hw):
+        """Output head, then eps in NCHW: its first out-channel columns (the planes pad the conv's N to 4)."""
+        o = self.out_head(norm, conv, h, hw)
+        out = torch.zeros((self.B, o.cols, hw[0], hw[1]), dtype=torch.float32, device=self.dev)
+        self.keep.append(out)
+        self.misc(_lib.QD_OP_NHWC_TO_NCHW, o.ptr, out.data_ptr(), self.B, o.cols, hw[0] * hw[1], label="eps.nchw",
+                  spec=dict(kind="nhwc_to_nchw", src=o, dst=out))
+        return out[:, :int(conv.weight.shape[0])]
+
+    def lower_ldm(self, model, x_shape, ctx_shape, cfg_dedup=False):
+        """UNetModel.forward (openaimodel.py:745-782) in every state: the blocks, linear_f32, conv_f32 and out_head are
+        this builder's own.  cfg_dedup: x_shape / ctx_shape describe the doubled classifier-free-guidance batch, and the
+        guidance-invariant prefix is recorded for the first half only (cfg_split)."""
+        if cfg_dedup:
+            if x_shape[0] % 2 or ctx_shape is None or ctx_shape[0] != x_shape[0]:
+                raise ValueError("cfg_dedup needs an even batch [uncond; cond] with one context row per sample")
+            self.B, self.prefix = x_shape[0] // 2, True
+        x_in, t_in, ctx_in, emb, h = self._prologue(x_shape, ctx_shape, model.model_channels, 0, model.time_embed[0],
+                                                    model.time_embed[2])
+        ctx = None
+        if ctx_in is not None:
+            ctx = (Act(ctx_in, ctx_shape[0] * ctx_shape[1], ctx_shape[2]), ctx_shape[1])
+        hw = tuple(x_shape[2:])
         hs = []
         self.cfg_live = [emb]             # tensors the prefix hands over to the full batch (plus the skips, appended below)
 
@@ -947,7 +981,7 @@ class Builder:
 
         def dest_view(j, side, cs, ohw):
             """View for decoder block j's concat: side 'skip' = right-hand columns, 'h' = left-hand ones."""
-            if j is None or j < 0 or j >= nblk or cat_total[j] is None:
+            if not self.concat_in_place or j is None or j < 0 or j >= nblk or cat_total[j] is None:
                 return None
             rows = self.B * ohw[0] * ohw[1]
             if cat_buf[j] is None:
@@ -973,9 +1007,7 @@ class Builder:
                 if dest is not None and li == len(seq) - 1:
                     out = dest_view(dest[0], dest[1], last_out_channels(layer, h.cols), last_out_hw(layer, hw))
                 if n == "QuantModule":                       # conv_in
-                    a = self.quantize(h, layer.act_quantizer, self.key(layer) + ".q")
-                    kt = (9 * h.cols + 31) // 32 * 32
-                    h = self.conv_im2col(layer, a, hw, self.key(layer), 1, (1, 1), hw, kt, out=out)
+                    h, hw = self.conv_f32(layer, h, hw, self.key(layer), out=out)
                 elif n in _RES:
                     h, hw = self.ldm_resblock(layer, h, emb, hw, split, out=out)
                 elif n in _ST:
@@ -983,25 +1015,17 @@ class Builder:
                 elif n in _ATTN:
                     h = self.ldm_attention_block(layer, h, hw, out=out)
                 elif n == "Downsample":
-                    op = layer.op
-                    if _name(op) != "QuantModule":
+                    if _name(layer.op) != "QuantModule":
                         raise NotImplementedError("Downsample without conv")
-                    a = self.quantize(h, op.act_quantizer, self.key(op) + ".q")
-                    ohw = (hw[0] // 2, hw[1] // 2)
-                    h = self.conv_im2col(op, a, hw, self.key(op), 2, (1, 1), ohw, 9 * h.cols, out=out)
-                    hw = ohw
+                    h, hw = self.conv_f32(layer.op, h, hw, self.key(layer.op), stride=2, out=out)
                 elif n == "Upsample":
-                    conv = layer.conv
-                    a = self.quantize(h, conv.act_quantizer, self.key(conv) + ".q", upsample=(self.B, hw[0], hw[1]))
-                    hw = (2 * hw[0], 2 * hw[1])
-                    h = self.conv3x3_s1(conv, a, hw, self.key(conv), out=out)
+                    h, hw = self.conv_f32(layer.conv, h, hw, self.key(layer.conv), upsample=True, out=out)
                 else:
                     raise NotImplementedError(f"unhandled layer type {n} at {self.key(layer)}")
             return h, hw
 
         nin_blocks = len(model.input_blocks)
         for i, blk in enumerate(model.input_blocks):
-            B = self.B                    # half batch inside the guidance prefix, full batch after cfg_split
             h, hw = run(blk, h, hw, 0, dest=(nin_blocks - 1 - i, "skip") if nin_blocks == nblk else None)
             hs.append((h, hw))
             if self.prefix:
@@ -1009,7 +1033,6 @@ class Builder:
             self.traces[f"input_blocks.{i}"] = (h, hw)
         if self.prefix:
             raise NotImplementedError("cfg_dedup: no cross-attention found to end the guidance-invariant prefix")
-        B = self.B
         h, hw = run(model.middle_block, h, hw, 0, dest=(0, "h"))
         self.traces["middle_block"] = (h, hw)
         for i, blk in enumerate(model.output_blocks):
@@ -1023,14 +1046,7 @@ class Builder:
                 h = self.concat(h, skip_t, f"output_blocks.{i}")
             h, hw = run(blk, h, hw, split, dest=(i + 1, "h"))
             self.traces[f"output_blocks.{i}"] = (h, hw)
-        norm, conv = model.out[0], model.out[2]
-        (a,), _ = self.groupnorm(h, norm, hw[0] * hw[1], [conv.act_quantizer], True, "out.0")
-        o = self.conv3x3_s1(conv, a, hw, "out.2")
-        out = torch.zeros((B, o.cols, hw[0], hw[1]), dtype=torch.float32, device=self.dev)
-        self.keep.append(out)
-        self.misc(_lib.QD_OP_NHWC_TO_NCHW, o.ptr, out.data_ptr(), B, o.cols, hw[0] * hw[1], label="eps.nchw",
-                  spec=dict(kind="nhwc_to_nchw", src=o, dst=out))
-        return x_in, t_in, ctx_in, out
+        return x_in, t_in, ctx_in, self._epilogue(model.out[0], model.out[2], h, hw)
 
     # ================================================================== DDIM (CIFAR) family
     def ddim_resnet(self, blk, x, temb, hw, split, out=None):
@@ -1041,7 +1057,7 @@ class Builder:
         if has_nin and getattr(blk, "use_conv_shortcut", False):
             raise NotImplementedError("conv_shortcut=True is not used by the reference configs")
         a_skip = None
-        if has_nin and split % 4 == 0 and os.environ.get("QDIFF_DDIM_NINQ", "fused") != "separate":
+        if has_nin and split % 4 == 0:
             # nin_shortcut's (split) input quantizer reads the tensor norm1 reads: emitted by the same GroupNorm pass
             nin = blk.nin_shortcut
             if split and nin.split == 0:
@@ -1050,7 +1066,7 @@ class Builder:
             (a1,), _, a_skip = self.groupnorm(x, blk.norm1, H * W, [blk.conv1.act_quantizer], True, k + ".norm1", raw=raw)
         else:
             (a1,), _ = self.groupnorm(x, blk.norm1, H * W, [blk.conv1.act_quantizer], True, k + ".norm1")
-        tp = self.qlinear(blk.temb_proj, temb, k + ".temb_proj", act=1)
+        tp = self.linear_f32(blk.temb_proj, temb, k + ".temb_proj", act=1)
         h = self.conv3x3_s1(blk.conv1, a1, hw, k + ".conv1", rowvec=tp)
         (a2,), _ = self.groupnorm(h, blk.norm2, H * W, [blk.conv2.act_quantizer], True, k + ".norm2")
         s = x
@@ -1067,7 +1083,7 @@ class Builder:
             elif a_skip is not None:
                 s = self.gemm(nin, a_skip, k + ".nin_shortcut")
             else:
-                s = self.qlinear(nin, x, k + ".nin_shortcut")
+                s = self.linear_f32(nin, x, k + ".nin_shortcut")
         return self.conv3x3_s1(blk.conv2, a2, hw, k + ".conv2", residual=s, out=out)
 
     def ddim_attn(self, blk, x, hw, out=None):
@@ -1087,33 +1103,23 @@ class Builder:
         return self.gemm(blk.proj_out, o, k + ".proj_out", residual=x, out=out)
 
     def lower_ddim(self, model, x_shape):
-        B, Cin, H, W = x_shape
-        x_in = torch.zeros(x_shape, dtype=torch.float32, device=self.dev)
-        t_in = torch.zeros(B, dtype=torch.float32, device=self.dev)
-        self.keep += [x_in, t_in]
+        """Model.forward (ddim/models/diffusion.py:308-360) in every state, like lower_ldm."""
+        x_in, t_in, _, temb, h = self._prologue(x_shape, None, model.ch, 1, model.temb.dense[0], model.temb.dense[1])
+        B = self.B
         split_on = bool(getattr(model.config, "split_shortcut", False))
-        temb0 = self.new_f32(B, model.ch)
-        self.misc(_lib.QD_OP_TIMESTEP_EMB, t_in.data_ptr(), temb0.ptr, B, model.ch, 1, label="timestep_embedding",
-                  aux=ops.timestep_freqs(model.ch, 1).to(self.dev), spec=dict(kind="timestep_emb", t=t_in, dst=temb0, mode=1))
-        e = self.qlinear(model.temb.dense[0], temb0, "temb.dense.0")
-        temb = self.qlinear(model.temb.dense[1], e, "temb.dense.1", act=1)
-        xh = self.new_f32(B * H * W, Cin)
-        self.misc(_lib.QD_OP_NCHW_TO_NHWC, x_in.data_ptr(), xh.ptr, B, Cin, H * W, label="x.nhwc",
-                  spec=dict(kind="nchw_to_nhwc", src=x_in, dst=xh))
         nres = model.num_resolutions
         # torch.cat([h, hs.pop()], dim=1) without copies (ddim/models/diffusion.py:346): decoder block u (in execution order)
         # consumes the u-th last skip.  Its concat buffer is allocated when that skip is produced - the producer's last GEMM
         # writes the right-hand columns - and whatever produces h for block u (mid.block_2, the previous decoder block, an
-        # upsample conv) writes the left-hand ones.  QDIFF_DDIM_CAT=copy restores the two copies per block (A/B switch).
+        # upsample conv) writes the left-hand ones.
         up_blocks = [model.up[lv].block[ib] for lv in reversed(range(nres)) for ib in range(model.num_res_blocks + 1)]
         n_hs = len(up_blocks)
         cat_buf = [None] * n_hs
-        in_place = os.environ.get("QDIFF_DDIM_CAT", "inplace") != "copy"
 
         def skip_view(i_hs, cs, rows):
             """Right-hand columns of the concat buffer of the decoder block that will pop skip number i_hs."""
             u = n_hs - 1 - i_hs
-            total = int(up_blocks[u].in_channels) if in_place and 0 <= u < n_hs else 0
+            total = int(up_blocks[u].in_channels) if self.concat_in_place and 0 <= u < n_hs else 0
             if total <= cs or total % 4 or cs % 4:
                 return None
             cat_buf[u] = self.new_f32(rows, total)
@@ -1126,10 +1132,9 @@ class Builder:
                 return None
             return buf.view(0, ch)
 
-        a = self.quantize(xh, model.conv_in.act_quantizer, "conv_in.q")
-        hw = (H, W)
-        h = self.conv_im2col(model.conv_in, a, hw, "conv_in", 1, (1, 1), hw, (9 * Cin + 31) // 32 * 32,
-                             out=skip_view(0, int(model.conv_in.weight.shape[0]), B * H * W))
+        hw = tuple(x_shape[2:])
+        h, hw = self.conv_f32(model.conv_in, h, hw, "conv_in",
+                              out=skip_view(0, int(model.conv_in.weight.shape[0]), B * hw[0] * hw[1]))
         hs = [(h, hw)]
         for lv in range(nres):
             st = model.down[lv]
@@ -1143,12 +1148,10 @@ class Builder:
                 hs.append((h, hw))
             if lv != nres - 1:
                 conv = st.downsample.conv
-                a = self.quantize(hs[-1][0], conv.act_quantizer, self.key(conv) + ".q")
                 ohw = (hw[0] // 2, hw[1] // 2)
                 # F.pad (0,1,0,1) then 3x3 stride 2, padding 0 (ddim/models/diffusion.py:67-71)
-                h = self.conv_im2col(conv, a, hw, self.key(conv), 2, (0, 0), ohw, 9 * a.cols,
-                                     out=skip_view(len(hs), int(conv.weight.shape[0]), B * ohw[0] * ohw[1]))
-                hw = ohw
+                h, hw = self.conv_f32(conv, hs[-1][0], hw, self.key(conv), stride=2, pad_tl=(0, 0),
+                                      out=skip_view(len(hs), int(conv.weight.shape[0]), B * ohw[0] * ohw[1]))
                 hs.append((h, hw))
         h = hs[-1][0]
         h = self.ddim_resnet(model.mid.block_1, h, temb, hw, 0)
@@ -1179,17 +1182,9 @@ class Builder:
                 u += 1
             if lv != 0:
                 conv = st.upsample.conv
-                a = self.quantize(h, conv.act_quantizer, self.key(conv) + ".q", upsample=(B, hw[0], hw[1]))
-                hw = (2 * hw[0], 2 * hw[1])
-                h = self.conv3x3_s1(conv, a, hw, self.key(conv),
-                                    out=h_view(u, int(conv.weight.shape[0]), B * hw[0] * hw[1]))
-        (a,), _ = self.groupnorm(h, model.norm_out, hw[0] * hw[1], [model.conv_out.act_quantizer], True, "norm_out")
-        o = self.conv3x3_s1(model.conv_out, a, hw, "conv_out")
-        out = torch.zeros((B, o.cols, hw[0], hw[1]), dtype=torch.float32, device=self.dev)
-        self.keep.append(out)
-        self.misc(_lib.QD_OP_NHWC_TO_NCHW, o.ptr, out.data_ptr(), B, o.cols, hw[0] * hw[1], label="eps.nchw",
-                  spec=dict(kind="nhwc_to_nchw", src=o, dst=out))
-        return x_in, t_in, None, out
+                h, hw = self.conv_f32(conv, h, hw, self.key(conv), upsample=True,
+                                      out=h_view(u, int(conv.weight.shape[0]), 4 * B * hw[0] * hw[1]))
+        return x_in, t_in, None, self._epilogue(model.norm_out, model.conv_out, h, hw)
 
 
 # ====================================================================== bfloat16-plane lowering (quant_act False)
@@ -1212,6 +1207,7 @@ class WeightOnlyBuilder(Builder):
     The first stage and the text encoder lower their floating-point GEMMs through the same recorder (plane_gemm)."""
 
     precision = None    # plane products of fp32 weights (_PASSES); None: each QuantModule's state picks codes or six
+    concat_in_place = False     # the decoder concat is copied (two copy2d ops per block)
 
     def split3(self, src, label, act=0, upsample=None, cols=None):
         C_ = src.cols if cols is None else cols
@@ -1339,9 +1335,23 @@ class WeightOnlyBuilder(Builder):
         self.layer_traces[label] = o
         return o
 
-    def lin(self, qm, x_f32, label, act=0, **kw):
+    def linear_f32(self, qm, x_f32, label, act=0, **kw):
         cols = x_f32.cols // 2 if act == 2 else None
         return self.plane_gemm(qm, self.split3(x_f32, label + ".split", act=act, cols=cols), label, **kw)
+
+    def conv_f32(self, qm, x, hw, label, stride=1, pad_tl=(1, 1), upsample=False, out=None):
+        """Builder.conv_f32 on bfloat16 planes."""
+        if upsample:
+            a = self.split3(x, label + ".split", upsample=(self.B, hw[0], hw[1]))
+            hw = (2 * hw[0], 2 * hw[1])
+            return self.plane_gemm(qm, a, label, hw=hw, rows_per_batch=hw[0] * hw[1], out=out), hw
+        ohw = (hw[0] // stride, hw[1] // stride)
+        return self.plane_gemm(qm, self.split3(x, label + ".split"), label, im2col=(hw, stride, pad_tl, ohw), out=out), ohw
+
+    def out_head(self, norm, conv, h, hw):
+        hn = self.gn_f32(h, norm, hw[0] * hw[1], True, self.key(norm))
+        return self.plane_gemm(conv, self.split3(hn, self.key(conv) + ".split"), self.key(conv), hw=hw,
+                               rows_per_batch=hw[0] * hw[1])
 
     def ln_f32(self, x, norm, label):
         """nn.LayerNorm with fp32 output (qd_layernorm_quant, n_out = 0)."""
@@ -1384,15 +1394,15 @@ class WeightOnlyBuilder(Builder):
             self.plane_gemm(qm, self.split3(x.view(split, x.cols - split), label + ".split1"), label, cols=(split, x.cols),
                          suffix="_0", accumulate_into=s, use_bias=False)
             return s
-        return self.lin(qm, x, label)
+        return self.linear_f32(qm, x, label)
 
     # ================================================================== DDIM (CIFAR) family
-    def ddim_resnet(self, blk, x, temb, hw, split):
+    def ddim_resnet(self, blk, x, temb, hw, split, out=None):
         """QuantResnetBlock.forward (qdiff/quant_block.py:307-330) with use_act_quant False."""
         k = self.key(blk)
         H, W = hw
         h1 = self.gn_f32(x, blk.norm1, H * W, True, k + ".norm1")
-        tp = self.lin(blk.temb_proj, temb, k + ".temb_proj", act=1)
+        tp = self.linear_f32(blk.temb_proj, temb, k + ".temb_proj", act=1)
         h = self.plane_gemm(blk.conv1, self.split3(h1, k + ".conv1.split"), k + ".conv1", hw=(H, W),
                          rows_per_batch=H * W, rowvec=tp)
         h2 = self.gn_f32(h, blk.norm2, H * W, True, k + ".norm2")
@@ -1402,9 +1412,9 @@ class WeightOnlyBuilder(Builder):
                 raise NotImplementedError("conv_shortcut=True is not used by the reference configs")
             s = self.shortcut(blk.nin_shortcut, x, k + ".nin_shortcut", split)
         return self.plane_gemm(blk.conv2, self.split3(h2, k + ".conv2.split"), k + ".conv2", hw=(H, W),
-                            rows_per_batch=H * W, residual=s)
+                               rows_per_batch=H * W, residual=s, out=out)
 
-    def ddim_attn(self, blk, x, hw):
+    def ddim_attn(self, blk, x, hw, out=None):
         """QuantAttnBlock.forward (qdiff/quant_block.py:354-386) with use_act_quant False: plain fp32 attention."""
         k = self.key(blk)
         T = hw[0] * hw[1]
@@ -1416,71 +1426,10 @@ class WeightOnlyBuilder(Builder):
         v = self.plane_gemm(blk.v, a, k + ".v")
         o = self.attention_fp(q, kk, v, heads=1, d=C_, Tq=T, Tk=T, q_layout=(0, C_), k_layout=(0, C_), v_layout=(0, C_),
                               scale=float(int(C_) ** (-0.5)), label=k + ".attn")
-        return self.lin(blk.proj_out, o, k + ".proj_out", residual=x)
-
-    def lower_ddim(self, model, x_shape):
-        B, Cin, H, W = x_shape
-        x_in = torch.zeros(x_shape, dtype=torch.float32, device=self.dev)
-        t_in = torch.zeros(B, dtype=torch.float32, device=self.dev)
-        self.keep += [x_in, t_in]
-        split_on = bool(getattr(model.config, "split_shortcut", False))
-        temb0 = self.new_f32(B, model.ch)
-        self.misc(_lib.QD_OP_TIMESTEP_EMB, t_in.data_ptr(), temb0.ptr, B, model.ch, 1, label="timestep_embedding",
-                  aux=ops.timestep_freqs(model.ch, 1).to(self.dev), spec=dict(kind="timestep_emb", t=t_in, dst=temb0, mode=1))
-        e = self.lin(model.temb.dense[0], temb0, "temb.dense.0")
-        temb = self.lin(model.temb.dense[1], e, "temb.dense.1", act=1)
-        xh = self.new_f32(B * H * W, Cin)
-        self.misc(_lib.QD_OP_NCHW_TO_NHWC, x_in.data_ptr(), xh.ptr, B, Cin, H * W, label="x.nhwc",
-                  spec=dict(kind="nchw_to_nhwc", src=x_in, dst=xh))
-        hw = (H, W)
-        h = self.plane_gemm(model.conv_in, self.split3(xh, "conv_in.split"), "conv_in", im2col=(hw, 1, (1, 1), hw))
-        hs = [(h, hw)]
-        nres = model.num_resolutions
-        for lv in range(nres):
-            st = model.down[lv]
-            for ib in range(model.num_res_blocks):
-                h = self.ddim_resnet(st.block[ib], hs[-1][0], temb, hw, 0)
-                if len(st.attn) > 0:
-                    h = self.ddim_attn(st.attn[ib], h, hw)
-                hs.append((h, hw))
-            if lv != nres - 1:
-                conv = st.downsample.conv
-                ohw = (hw[0] // 2, hw[1] // 2)
-                # F.pad (0,1,0,1) then 3x3 stride 2, padding 0 (ddim/models/diffusion.py:67-71)
-                h = self.plane_gemm(conv, self.split3(hs[-1][0], self.key(conv) + ".split"), self.key(conv),
-                                 im2col=(hw, 2, (0, 0), ohw))
-                hw = ohw
-                hs.append((h, hw))
-        h = hs[-1][0]
-        h = self.ddim_resnet(model.mid.block_1, h, temb, hw, 0)
-        h = self.ddim_attn(model.mid.attn_1, h, hw)
-        h = self.ddim_resnet(model.mid.block_2, h, temb, hw, 0)
-        self.traces["mid"] = (h, hw)
-        for lv in reversed(range(nres)):
-            st = model.up[lv]
-            for ib in range(model.num_res_blocks + 1):
-                split = h.cols if (lv < 4 and split_on) else 0
-                skip_t, _ = hs.pop()
-                cat = self.concat(h, skip_t, f"up.{lv}.block.{ib}")
-                h = self.ddim_resnet(st.block[ib], cat, temb, hw, split)
-                if len(st.attn) > 0:
-                    h = self.ddim_attn(st.attn[ib], h, hw)
-            if lv != 0:
-                conv = st.upsample.conv
-                a = self.split3(h, self.key(conv) + ".split", upsample=(B, hw[0], hw[1]))
-                hw = (2 * hw[0], 2 * hw[1])
-                h = self.plane_gemm(conv, a, self.key(conv), hw=hw, rows_per_batch=hw[0] * hw[1])
-        hn = self.gn_f32(h, model.norm_out, hw[0] * hw[1], True, "norm_out")
-        o = self.plane_gemm(model.conv_out, self.split3(hn, "conv_out.split"), "conv_out", hw=hw,
-                         rows_per_batch=hw[0] * hw[1])
-        out = torch.zeros((B, o.cols, hw[0], hw[1]), dtype=torch.float32, device=self.dev)   # o.cols: out_ch padded to 4
-        self.keep.append(out)
-        self.misc(_lib.QD_OP_NHWC_TO_NCHW, o.ptr, out.data_ptr(), B, o.cols, hw[0] * hw[1], label="eps.nchw",
-                  spec=dict(kind="nhwc_to_nchw", src=o, dst=out))
-        return x_in, t_in, None, out[:, :int(model.conv_out.weight.shape[0])]
+        return self.linear_f32(blk.proj_out, o, k + ".proj_out", residual=x, out=out)
 
     # ================================================================== LDM / SD family
-    def wo_resblock(self, blk, x, emb, hw, split):
+    def ldm_resblock(self, blk, x, emb, hw, split, out=None):
         """QuantResBlock._forward (qdiff/quant_block.py:83-111) with fp32 activations."""
         k = self.key(blk)
         H, W = hw
@@ -1507,7 +1456,7 @@ class WeightOnlyBuilder(Builder):
                           spec=dict(kind="avgpool2x", src=x, dst=x_res, B=self.B, H=H, W=W))
         else:
             a1 = self.split3(h1, k + ".in_layers.2.split")
-        emb_out = self.lin(blk.emb_layers[1], emb, k + ".emb_layers.1", act=1)
+        emb_out = self.linear_f32(blk.emb_layers[1], emb, k + ".emb_layers.1", act=1)
         oc = int(conv2.weight.shape[0])
         if getattr(blk, "use_scale_shift_norm", False):
             h = self.plane_gemm(conv1, a1, k + ".in_layers.2", hw=(oh, ow), rows_per_batch=oh * ow)
@@ -1523,44 +1472,44 @@ class WeightOnlyBuilder(Builder):
                 raise NotImplementedError("3x3 skip_connection (use_conv=True) is not used by any reference config")
             s_ = self.shortcut(skip, x_res, k + ".skip_connection", split)
         out = self.plane_gemm(conv2, self.split3(h2, k + ".out_layers.3.split"), k + ".out_layers.3", hw=(oh, ow),
-                           rows_per_batch=oh * ow, residual=s_)
+                              rows_per_batch=oh * ow, residual=s_, out=out)
         return out, (oh, ow)
 
-    def wo_cross_attention(self, attn, xq, xkv, h_res, Tq, Tk, label):
+    def cross_attention_fp(self, attn, xq, xkv, h_res, Tq, Tk, label):
         """cross_attn_forward (qdiff/quant_block.py:190-221) with use_act_quant False: plain fp32 attention."""
         heads = attn.heads
         inner = int(attn.to_q.weight.shape[0])
         d = inner // heads
-        q = self.lin(attn.to_q, xq, label + ".to_q")
+        q = self.linear_f32(attn.to_q, xq, label + ".to_q")
         a_kv = self.split3(xkv, label + ".kv.split")
         kk = self.plane_gemm(attn.to_k, a_kv, label + ".to_k")
         v = self.plane_gemm(attn.to_v, a_kv, label + ".to_v")
         o = self.attention_fp(q, kk, v, heads=heads, d=d, Tq=Tq, Tk=Tk, q_layout=(0, d), k_layout=(0, d), v_layout=(0, d),
                               scale=float(attn.scale), label=label + ".attn")
-        return self.lin(attn.to_out[0], o, label + ".to_out.0", residual=h_res)
+        return self.linear_f32(attn.to_out[0], o, label + ".to_out.0", residual=h_res)
 
-    def wo_spatial_transformer(self, st, x, ctx, hw):
+    def spatial_transformer(self, st, x, ctx, hw, out=None):
         """SpatialTransformer.forward (ldm/modules/attention.py:276-287) + QuantBasicTransformerBlock._forward
         (qdiff/quant_block.py:263-271), fp32 activations."""
         k = self.key(st)
         T = hw[0] * hw[1]
         hn = self.gn_f32(x, st.norm, T, False, k + ".norm")
-        h = self.lin(st.proj_in, hn, k + ".proj_in")
+        h = self.linear_f32(st.proj_in, hn, k + ".proj_in")
         if ctx is None:
             raise ValueError("SpatialTransformer needs a context tensor")
         ctx_act, Tk = ctx
         for i, blk in enumerate(st.transformer_blocks):
             bk = f"{k}.transformer_blocks.{i}"
             n1 = self.ln_f32(h, blk.norm1, bk + ".norm1")
-            h = self.wo_cross_attention(blk.attn1, n1, n1, h, T, T, bk + ".attn1")
+            h = self.cross_attention_fp(blk.attn1, n1, n1, h, T, T, bk + ".attn1")
             n2 = self.ln_f32(h, blk.norm2, bk + ".norm2")
-            h = self.wo_cross_attention(blk.attn2, n2, ctx_act, h, T, Tk, bk + ".attn2")
+            h = self.cross_attention_fp(blk.attn2, n2, ctx_act, h, T, Tk, bk + ".attn2")
             n3 = self.ln_f32(h, blk.norm3, bk + ".norm3")
-            f = self.lin(blk.ff.net[0].proj, n3, bk + ".ff.net.0.proj")
-            h = self.lin(blk.ff.net[2], f, bk + ".ff.net.2", act=2, residual=h)      # GEGLU inside the plane split
-        return self.lin(st.proj_out, h, k + ".proj_out", residual=x)
+            f = self.linear_f32(blk.ff.net[0].proj, n3, bk + ".ff.net.0.proj")
+            h = self.linear_f32(blk.ff.net[2], f, bk + ".ff.net.2", act=2, residual=h)      # GEGLU inside the plane split
+        return self.linear_f32(st.proj_out, h, k + ".proj_out", residual=x, out=out)
 
-    def wo_attention_block(self, blk, x, hw):
+    def ldm_attention_block(self, blk, x, hw, out=None):
         """AttentionBlock._forward + QKVAttentionLegacy (openaimodel.py:321-327,384-406) in fp32: the qkv conv output
         [B*T, heads * 3 * ch] is addressed in place (head h: q at 3*ch*h, k at +ch, v at +2*ch); (q s)(k s) = q k / sqrt(ch)."""
         k = self.key(blk)
@@ -1568,80 +1517,10 @@ class WeightOnlyBuilder(Builder):
         heads = blk.attention.n_heads
         ch = C_ // heads
         hn = self.gn_f32(x, blk.norm, T, False, k + ".norm")
-        qkv = self.lin(blk.qkv, hn, k + ".qkv")
+        qkv = self.linear_f32(blk.qkv, hn, k + ".qkv")
         o = self.attention_fp(qkv, qkv, qkv, heads=heads, d=ch, Tq=T, Tk=T, q_layout=(0, 3 * ch), k_layout=(ch, 3 * ch),
                               v_layout=(2 * ch, 3 * ch), scale=1.0 / math.sqrt(ch), label=k + ".attention")
-        return self.lin(blk.proj_out, o, k + ".proj_out", residual=x)
-
-    def lower_ldm(self, model, x_shape, ctx_shape):
-        """UNetModel.forward (openaimodel.py:745-782) with fp32 activations (weight-only and full-precision states)."""
-        B, Cin, H, W = x_shape
-        x_in = torch.zeros(x_shape, dtype=torch.float32, device=self.dev)
-        t_in = torch.zeros(B, dtype=torch.float32, device=self.dev)
-        ctx_in = torch.zeros(ctx_shape, dtype=torch.float32, device=self.dev) if ctx_shape is not None else None
-        self.keep += [x_in, t_in] + ([ctx_in] if ctx_in is not None else [])
-        mc = model.model_channels
-        temb = self.new_f32(B, mc)
-        self.misc(_lib.QD_OP_TIMESTEP_EMB, t_in.data_ptr(), temb.ptr, B, mc, 0, label="timestep_embedding",
-                  aux=ops.timestep_freqs(mc, 0).to(self.dev), spec=dict(kind="timestep_emb", t=t_in, dst=temb, mode=0))
-        e = self.lin(model.time_embed[0], temb, "time_embed.0")
-        emb = self.lin(model.time_embed[2], e, "time_embed.2", act=1)
-        ctx = None
-        if ctx_in is not None:
-            ctx = (Act(ctx_in, ctx_shape[0] * ctx_shape[1], ctx_shape[2]), ctx_shape[1])
-        xh = self.new_f32(B * H * W, Cin)
-        self.misc(_lib.QD_OP_NCHW_TO_NHWC, x_in.data_ptr(), xh.ptr, B, Cin, H * W, label="x.nhwc",
-                  spec=dict(kind="nchw_to_nhwc", src=x_in, dst=xh))
-
-        def run(seq, h, hw, split):
-            for layer in seq:
-                n = _name(layer)
-                if n == "QuantModule":                       # conv_in
-                    h = self.plane_gemm(layer, self.split3(h, self.key(layer) + ".split"), self.key(layer),
-                                     im2col=(hw, 1, (1, 1), hw))
-                elif n in _RES:
-                    h, hw = self.wo_resblock(layer, h, emb, hw, split)
-                elif n in _ST:
-                    h = self.wo_spatial_transformer(layer, h, ctx, hw)
-                elif n in _ATTN:
-                    h = self.wo_attention_block(layer, h, hw)
-                elif n == "Downsample":
-                    op = layer.op
-                    if _name(op) != "QuantModule":
-                        raise NotImplementedError("Downsample without conv")
-                    ohw = (hw[0] // 2, hw[1] // 2)
-                    h = self.plane_gemm(op, self.split3(h, self.key(op) + ".split"), self.key(op), im2col=(hw, 2, (1, 1), ohw))
-                    hw = ohw
-                elif n == "Upsample":
-                    conv = layer.conv
-                    a = self.split3(h, self.key(conv) + ".split", upsample=(self.B, hw[0], hw[1]))
-                    hw = (2 * hw[0], 2 * hw[1])
-                    h = self.plane_gemm(conv, a, self.key(conv), hw=hw, rows_per_batch=hw[0] * hw[1])
-                else:
-                    raise NotImplementedError(f"unhandled layer type {n} at {self.key(layer)}")
-            return h, hw
-
-        h, hw, hs = xh, (H, W), []
-        for i, blk in enumerate(model.input_blocks):
-            h, hw = run(blk, h, hw, 0)
-            hs.append((h, hw))
-            self.traces[f"input_blocks.{i}"] = (h, hw)
-        h, hw = run(model.middle_block, h, hw, 0)
-        self.traces["middle_block"] = (h, hw)
-        for i, blk in enumerate(model.output_blocks):
-            skip_t, _ = hs.pop()
-            split = h.cols if getattr(model, "split", False) else 0
-            h = self.concat(h, skip_t, f"output_blocks.{i}")
-            h, hw = run(blk, h, hw, split)
-            self.traces[f"output_blocks.{i}"] = (h, hw)
-        hn = self.gn_f32(h, model.out[0], hw[0] * hw[1], True, "out.0")
-        o = self.plane_gemm(model.out[2], self.split3(hn, "out.2.split"), "out.2", hw=hw,
-                         rows_per_batch=hw[0] * hw[1])
-        out = torch.zeros((B, o.cols, hw[0], hw[1]), dtype=torch.float32, device=self.dev)   # o.cols: out channels padded to 4
-        self.keep.append(out)
-        self.misc(_lib.QD_OP_NHWC_TO_NCHW, o.ptr, out.data_ptr(), B, o.cols, hw[0] * hw[1], label="eps.nchw",
-                  spec=dict(kind="nhwc_to_nchw", src=o, dst=out))
-        return x_in, t_in, ctx_in, out[:, :int(model.out[2].weight.shape[0])]
+        return self.linear_f32(blk.proj_out, o, k + ".proj_out", residual=x, out=out)
 
 
 class _RowView:
@@ -1707,11 +1586,10 @@ def compile_unet(qnn, x_shape, ctx_shape, device, use_cuda_graph=True, cfg_dedup
             f"got mixed states {states}")
     model = qnn.model
     with torch.no_grad():
-        if cfg_dedup and (_name(model) != "UNetModel" or type(b) is not Builder):
+        if cfg_dedup and (_name(model) != "UNetModel" or isinstance(b, WeightOnlyBuilder)):
             raise NotImplementedError("cfg_dedup applies to the quantised LDM / SD UNets with a cross-attention context")
         if _name(model) == "UNetModel":
-            x_in, t_in, ctx_in, out = b.lower_ldm(model, x_shape, ctx_shape, cfg_dedup) if cfg_dedup else \
-                b.lower_ldm(model, x_shape, ctx_shape)
+            x_in, t_in, ctx_in, out = b.lower_ldm(model, x_shape, ctx_shape, cfg_dedup)
         elif _name(model) == "Model":
             x_in, t_in, ctx_in, out = b.lower_ddim(model, x_shape)
         else:

@@ -192,15 +192,32 @@ def main():
             lower = (lambda: b.lower_ddim(qnn.model, x_shape)) if g["family"] == "ddim" else \
                 (lambda: b.lower_ldm(qnn.model, x_shape, ctx_shape))
             record(f"{name}{'' if size is None else f' {size}x{size}'} state {state}", b, lower)
-    # ---- INT8 lowering of the DDIM family (concat-free decoder): op counts with and without the in-place concat
+    # ---- INT8 UNet programs: every quantised fixture at its own size and at 24x24 (the 3x3 convs take the patch gather),
+    # SD with the classifier-free-guidance prefix and with the context K/V recomputed every step
+    from tests.test_oracle_golden import CASES
+    for name in CASES:
+        g = load_case(name)
+        qnn = build_qnn(g, dev)
+        qnn.record_op_specs = True
+        ctx_shape = None if g["context"] is None else tuple(g["context"].shape)
+        variants = [(None, "", {}, False), (24, "", {}, False)]
+        if ctx_shape is not None:
+            variants += [(None, ", cfg_dedup", {}, True), (None, ", QDIFF_HOIST_CTX=0", {"QDIFF_HOIST_CTX": "0"}, False)]
+        for size, suffix, env, cfg_dedup in variants:
+            x_shape = tuple(g["x"].shape) if size is None else tuple(g["x"].shape[:2]) + (size, size)
+            os.environ.update(env)
+            b = graph.Builder(qnn, dev, x_shape[0])
+            lower = (lambda: b.lower_ddim(qnn.model, x_shape)) if g["family"] == "ddim" else \
+                (lambda: b.lower_ldm(qnn.model, x_shape, ctx_shape, cfg_dedup))
+            record(f"{name}{'' if size is None else f' {size}x{size}'} INT8{suffix}", b, lower,
+                   lambda r: f", {b.n_static} static, {sum(1 for k in b.op_kinds if k == _lib.QD_OP_COPY2D)} copy2d")
+            for k in env:
+                os.environ.pop(k)
+    # ---- the same DDIM program as compile_unet records it, without op specs (spec kinds "unspecified")
     g = load_case("ddim_w4a8_split")
     qnn = build_qnn(g, dev)
-    for mode in ("inplace", "copy"):
-        os.environ["QDIFF_DDIM_CAT"] = mode
-        b = graph.Builder(qnn, dev, g["x"].shape[0])
-        record(f"ddim_w4a8_split INT8, QDIFF_DDIM_CAT={mode}", b, lambda: b.lower_ddim(qnn.model, tuple(g["x"].shape)),
-               lambda r: f", {sum(1 for k in b.op_kinds if k == _lib.QD_OP_COPY2D)} copy2d")
-    os.environ.pop("QDIFF_DDIM_CAT", None)
+    b = graph.Builder(qnn, dev, g["x"].shape[0])
+    record("ddim_w4a8_split INT8, no op specs", b, lambda: b.lower_ddim(qnn.model, tuple(g["x"].shape)))
     # ---- CLIP text encoder (the tiny fixture's seeded weights)
     from oracle import clip_oracle
     gold = clip_oracle.load_tiny_fixture(os.path.join(ROOT, "tests", "golden", "clip_tiny.pt"))
