@@ -7,14 +7,21 @@
 // because the reference pads with real zeros AFTER de-quantisation, SURVEY Appendix A.3).
 //
 // Structure (one CTA per SM, persistent, warp-specialised):
-//   warp 0   : TMA producer  (A tile 128 x 128 B, B tile BN x 128 B, 128B swizzle, mbarrier ring); warp 1 idle
-//   warps 2-3 and the LAST two warps: INT4 unpack (W4 variant only: packed 4-bit weight codes staged by TMA -> swizzled
-//              s8 operand tile; four warps = one per scheduler)
-//   warps 4-11: two consumer warpgroups.  Warpgroup g issues wgmma m64nNk32 (int32 accumulators in registers) for rows
-//              [64g, 64g + 64) of the tile, the N tile as 64-column sub-blocks; after the K loop both warpgroups write
-//              their accumulators to a shared-memory tile, and the same eight warps run the epilogue from it
-//              (zero-point correction / scale / bias / adds / GEGLU -> coalesced fp32 or requantised stores).
-//   While the consumers run the epilogue, the producer already streams the next tile's operands into the ring.
+//   warps 0-3  : producer warpgroup.  Warp 0 is the TMA producer (A tile 128 x 128 B, B tile BN x 128 B, 128B swizzle,
+//                mbarrier ring); warp 1 initialises the barriers.  W4 variant: warps 2-3 and warps 12-13 unpack packed
+//                4-bit weight codes staged by TMA into the swizzled s8 operand tile (four warps = one per scheduler).
+//   warps 4-11 : two consumer warpgroups.  Warpgroup g issues wgmma m64nNk32 (int32 accumulators in registers) for rows
+//                [64g, 64g + 64) of the tile, the N tile as 64-column sub-blocks; after the K loop both warpgroups write
+//                their accumulators to a shared-memory accumulator tile.
+//   warps 12-  : gemm_epi_warps(MODE) epilogue warps (4 or 8) finalise the tile from there (zero-point correction / scale
+//                / bias / adds / GEGLU -> coalesced fp32 or requantised stores) while the consumers already run the next
+//                work item's k-blocks: two mbarriers (acc_full, acc_empty) hand the single accumulator tile back and
+//                forth, so a CTA's time per tile is the longer of main loop and epilogue rather than their sum.  Each role
+//                runs under its own register budget (setmaxnreg).
+//   Split-K partials (stored straight from the registers), packed INT4 weights, the bfloat16 weight-only layers and the
+//   generic MODE = -1 kernel keep the serial schedule: no epilogue warps, the eight consumer warps run the epilogue after
+//   each main loop.
+// The producer streams the next tile's operands into the ring while the current tile is finalised.
 //
 // The kernel is templated on the epilogue MODE so the hot variants carry no runtime flag tests
 // (a version with runtime flags was instruction-issue / I-cache bound in the epilogue).  MODE = -1 keeps every runtime
@@ -34,21 +41,6 @@ constexpr int GEMM_BK = 128;  // bytes == int8 elements per k-block (one 128B sw
 // (EPI_SPLITK) stores its raw accumulators straight from the registers, needs no accumulator tile and takes BN <= 256.
 constexpr int GEMM_MAX_BN = 128;
 constexpr int GEMM_MAX_BN_SPLITK = 256;
-// warps 0-3: TMA producer / idle (unpack warps 2-3 in the W4 variant); then the two consumer warpgroups (8 warps), which
-// are also the epilogue warps: warp (4 + 4h + q) finalises rows [32q, 32q + 32) of the tile, 32-column chunks h, h + 2, ...
-__host__ __device__ constexpr int gemm_epi_warps(int MODE) { return (void)MODE, 8; }
-// Residual operand through TMA: the plain-GEMM epilogues that add a residual (to_out / ff.net.2 / proj_out: EPI_RESIDUAL
-// without EPI_CONV) are bound by the latency of their residual loads when each warp issues 4 rows of LDG.128, waits a DRAM
-// round trip, stores, and issues the next 4 rows.
-// Now every epilogue warp owns a ring of GEMM_RES_NBUF 4 KB buffers and keeps the residual sub-tiles of its NEXT work items
-// (tile, chunk) in flight as cp.async.bulk.tensor loads while it finalises the current one.
-constexpr int GEMM_RES_NBUF = 3;
-__host__ __device__ constexpr bool gemm_res_tma(int MODE) { return MODE >= 0 && (MODE & 4) != 0 && (MODE & 256) != 0; }
-__host__ __device__ constexpr int gemm_res_bytes(int MODE) {
-  return gemm_res_tma(MODE) ? gemm_epi_warps(MODE) * GEMM_RES_NBUF * 4096 : 0;
-}
-// W4 (packed INT4 weights): two more warps behind the consumer warps join warps 2-3 as unpack warps
-__host__ __device__ constexpr int gemm_threads(int MODE, bool W4 = false) { return (4 + gemm_epi_warps(MODE) + (W4 ? 2 : 0)) * 32; }
 constexpr int GEMM_A_STAGE_BYTES = GEMM_BM * GEMM_BK;
 constexpr int GEMM_MAX_STAGES = 8;
 constexpr int GEMM_EPI_TILE_BYTES = 32 * 128;  // one 32 x 32 int32 chunk of the accumulator tile
@@ -71,6 +63,51 @@ constexpr int EPI_RESTMA = 256;   // with EPI_RESIDUAL: residual sub-tiles arriv
 constexpr int EPI_BF16 = 512;     // weight-only layers: bfloat16 x3 activation planes x bfloat16 weight codes, fp32 accumulators
 constexpr int EPI_SPLITK = 1024;  // split-K partial: raw int32 accumulators of one K slice -> ws[split][M][N] (splitk_finish_kernel applies the epilogue)
 __host__ __device__ constexpr int gemm_max_bn(int MODE) { return (MODE >= 0 && (MODE & EPI_SPLITK) != 0) ? GEMM_MAX_BN_SPLITK : GEMM_MAX_BN; }
+
+// Overlapped schedule (dedicated epilogue warps behind the consumers) for every specialised int8 epilogue.  Split-K partials
+// have no tile epilogue; packed INT4 weights, the bfloat16 weight-only layers and the generic MODE = -1 kernel (whose
+// run-time-flag epilogue spills hundreds of bytes as an epilogue role even at 232 registers) keep the serial schedule.
+__host__ __device__ constexpr bool gemm_overlap(int MODE, bool W4 = false) {
+  return MODE >= 0 && !W4 && (MODE & (EPI_SPLITK | EPI_BF16)) == 0;
+}
+// Epilogue warps: warp (4h + q) of them finalises rows [32q, 32q + 32) of the tile, 32-column chunks h, h + EPI_WARPS / 4,
+// ...  The 3x3 convs follow main loops of 20-180 k-blocks, so their epilogue is the shorter part of a tile: 4 warps at up
+// to 232 registers (border-class correction rows, per-image vectors).  The plain GEMMs' epilogues (short K: the epilogue
+// is the longer part) take 8 warps at 128 registers.  Serial schedule: the 8 consumer warps.
+__host__ __device__ constexpr int gemm_epi_warps(int MODE, bool W4 = false) {
+  return gemm_overlap(MODE, W4) && (MODE & EPI_CONV) != 0 ? 4 : 8;
+}
+// Registers per thread of each role on the overlapped schedule.  setmaxnreg only moves registers between the warps of
+// one CTA, so the budgets must fit the CTA's launch allocation, threads x (65,536 / threads rounded down to 8):
+//   8 epilogue warps (640 threads, 96 at launch: 61,440): producer warpgroup 32, consumers 96 (64 int32 accumulators at
+//     BN = 128 plus descriptors and ring state), epilogue warps 128 - 61,440;
+//   4 epilogue warps (512 threads, 128 at launch: 65,536): producer 32, consumers 104, epilogue warps 232 - 60,416.
+constexpr int GEMM_PRODUCER_REGS = 32;
+__host__ __device__ constexpr int gemm_consumer_regs(int MODE) { return gemm_epi_warps(MODE) == 8 ? 96 : 104; }
+__host__ __device__ constexpr int gemm_epi_regs(int MODE) { return gemm_epi_warps(MODE) == 8 ? 128 : 232; }
+// W4 (packed INT4 weights, serial schedule): warps 12-13 behind the consumer warps join warps 2-3 as unpack warps
+constexpr int GEMM_W4_WARP0 = 12;
+__host__ __device__ constexpr int gemm_threads(int MODE, bool W4 = false) {
+  return gemm_overlap(MODE, W4) ? (12 + gemm_epi_warps(MODE)) * 32 : (GEMM_W4_WARP0 + (W4 ? 2 : 0)) * 32;
+}
+__host__ __device__ constexpr int gemm_launch_regs(int MODE, bool W4 = false) { return (65536 / gemm_threads(MODE, W4)) & ~7; }
+// a warpgroup's move from the launch allocation FROM to R registers per thread
+template <int R, int FROM>
+__device__ __forceinline__ void gemm_setmaxnreg() {
+  if constexpr (R < FROM) setmaxnreg_dec<R>();
+  else if constexpr (R > FROM) setmaxnreg_inc<R>();
+}
+// Residual operand through TMA: the plain-GEMM epilogues that add a residual (to_out / ff.net.2 / proj_out: EPI_RESIDUAL
+// without EPI_CONV) are bound by the latency of their residual loads when each warp issues 4 rows of LDG.128, waits a DRAM
+// round trip, stores, and issues the next 4 rows.
+// Now every epilogue warp owns a ring of GEMM_RES_NBUF 4 KB buffers and keeps the residual sub-tiles of its NEXT work items
+// (tile, chunk) in flight as cp.async.bulk.tensor loads while it finalises the current one.  These modes take 8 epilogue
+// warps on either schedule.
+constexpr int GEMM_RES_NBUF = 3;
+__host__ __device__ constexpr bool gemm_res_tma(int MODE) { return MODE >= 0 && (MODE & EPI_RESIDUAL) != 0 && (MODE & EPI_RESTMA) != 0; }
+__host__ __device__ constexpr int gemm_res_bytes(int MODE) {
+  return gemm_res_tma(MODE) ? gemm_epi_warps(MODE) * GEMM_RES_NBUF * 4096 : 0;
+}
 
 struct GemmArgs {
   int M, N;            // logical output rows / columns (columns >= N are masked)
@@ -441,17 +478,24 @@ gemm_i8_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   const uint32_t pad = ((raw_addr + 1023u) & ~1023u) - raw_addr;
   uint8_t* smem = smem_raw + pad;
 
-  constexpr int EPI_WARPS = gemm_epi_warps(MODE);
+  constexpr bool OVL = gemm_overlap(MODE, W4);
+  constexpr int EPI_WARPS = gemm_epi_warps(MODE, W4);
   constexpr int CSTEP = 32 * (EPI_WARPS / 4);   // column stride between the chunks of one epilogue warp
   constexpr bool RES_TMA = gemm_res_tma(MODE);
   constexpr bool SPLITK = MODE >= 0 && (MODE & EPI_SPLITK) != 0;
   constexpr int NS = gemm_max_bn(MODE) / 64;     // 64-column accumulator sub-blocks
+  static_assert(!OVL || 128 * GEMM_PRODUCER_REGS + 256 * gemm_consumer_regs(MODE) + 32 * EPI_WARPS * gemm_epi_regs(MODE) <=
+                            gemm_threads(MODE) * gemm_launch_regs(MODE), "role register budgets exceed the CTA's allocation");
   const GemmSmemLayout lay = gemm_smem_layout(p.BN, p.stages, W4 ? 1 : 0, gemm_res_bytes(MODE), SPLITK);
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + lay.bar_offset);
   uint64_t* full_bar = bars;                          // [stages]
   uint64_t* empty_bar = bars + GEMM_MAX_STAGES;       // [stages] (one arrival per consumer warpgroup)
   uint64_t* ready_bar = bars + 2 * GEMM_MAX_STAGES;   // [stages] (w4: B tile unpacked, stage ready for the MMA)
   uint64_t* res_bar = bars + 3 * GEMM_MAX_STAGES;     // [EPI_WARPS][GEMM_RES_NBUF] (residual ring, RES_TMA only)
+  // overlapped schedule: the accumulator tile holds the current work item (one arrival per consumer warp) / the epilogue
+  // warps have finished reading it (one arrival per epilogue warp)
+  uint64_t* acc_full = bars + 3 * GEMM_MAX_STAGES + 8 * GEMM_RES_NBUF;
+  uint64_t* acc_empty = acc_full + 1;
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -469,117 +513,124 @@ gemm_i8_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   if (warp == 1 && lane == 0) {
     for (int s = 0; s < p.stages; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], EPI_WARPS / 4);
+      mbar_init(&empty_bar[s], 2);
       if constexpr (W4) mbar_init(&ready_bar[s], 4);    // one arrival per unpack warp
     }
     if constexpr (RES_TMA)
       for (int s = 0; s < EPI_WARPS * GEMM_RES_NBUF; ++s) mbar_init(&res_bar[s], 1);
+    if constexpr (OVL) {
+      mbar_init(acc_full, 8);
+      mbar_init(acc_empty, EPI_WARPS);
+    }
     fence_mbar_init();
     fence_proxy_async();
   }
   __syncthreads();
 
-  if (warp == 0) {
-    // ===================== TMA producer =====================
-    if (lane == 0) {
-      int stage = 0;
-      uint32_t phase = 0;
-      const uint32_t tx_bytes = (uint32_t)(GEMM_A_STAGE_BYTES + (W4 ? p.BN * (GEMM_BK / 2) : p.BN * GEMM_BK));
-      for (int item = blockIdx.x; item < num_tiles; item += gridDim.x) {
-        const int tile = item / splits;
-        const int kb0 = (item - tile * splits) * kb_slice;
-        const int kb1 = min(num_kb_all, kb0 + kb_slice);
-        const int tm = tile / p.tiles_n;
-        const int tn = tile - tm * p.tiles_n;
-        const int m0 = tm * GEMM_BM;
-        const int n0 = tn * p.BN;
-        int b0 = 0, h0 = 0, w0 = 0;
-        if (p.taps == 9) {
-          const int hw = p.H * p.W;
-          b0 = m0 / hw;
-          h0 = (m0 - b0 * hw) / p.W;
-          w0 = m0 - b0 * hw - h0 * p.W;      // != 0 only for rows wider than a tile (W > 128: the tile is a 128-pixel row segment)
-        }
-        int seg = kb0 / kb_per_tap, kc = kb0 - seg * kb_per_tap;
-        for (int kb = kb0; kb < kb1; ++kb) {
-          const int tap = seg % p.taps;            // activation geometry of this segment; the weight column offset is seg * C
-          const int ky = tap / 3, kx = tap - ky * 3;
-          {
-            mbar_wait(&empty_bar[stage], phase ^ 1);
-            uint8_t* sa = smem + (size_t)stage * lay.stage_bytes;
-            uint8_t* sb = sa + GEMM_A_STAGE_BYTES;
-            mbar_arrive_expect_tx(&full_bar[stage], tx_bytes);
-            if (p.taps == 9)
-              tma_load_4d(sa, &tmA, &full_bar[stage], kc * GEMM_BK, w0 + kx - 1, h0 + ky - 1, b0);
-            else
-              tma_load_4d(sa, &tmA, &full_bar[stage], kc * GEMM_BK, m0, 0, 0);
-            if constexpr (W4)
-              tma_load_2d(smem + lay.pack_off + (size_t)stage * p.BN * (GEMM_BK / 2), &tmB, &full_bar[stage],
-                          (seg * p.C + kc * GEMM_BK) / 2, n0);
-            else
-              tma_load_2d(sb, &tmB, &full_bar[stage], seg * p.C + kc * GEMM_BK, n0);
-            if (++stage == p.stages) { stage = 0; phase ^= 1; }
+  if (warp < 4 || (W4 && warp >= GEMM_W4_WARP0)) {
+    // ===================== producer warpgroup: TMA producer (warp 0), INT4 unpack (W4: warps 2-3 and 12-13) ============
+    if constexpr (OVL) gemm_setmaxnreg<GEMM_PRODUCER_REGS, gemm_launch_regs(MODE)>();
+    if (warp == 0) {
+      if (lane == 0) {
+        int stage = 0;
+        uint32_t phase = 0;
+        const uint32_t tx_bytes = (uint32_t)(GEMM_A_STAGE_BYTES + (W4 ? p.BN * (GEMM_BK / 2) : p.BN * GEMM_BK));
+        for (int item = blockIdx.x; item < num_tiles; item += gridDim.x) {
+          const int tile = item / splits;
+          const int kb0 = (item - tile * splits) * kb_slice;
+          const int kb1 = min(num_kb_all, kb0 + kb_slice);
+          const int tm = tile / p.tiles_n;
+          const int tn = tile - tm * p.tiles_n;
+          const int m0 = tm * GEMM_BM;
+          const int n0 = tn * p.BN;
+          int b0 = 0, h0 = 0, w0 = 0;
+          if (p.taps == 9) {
+            const int hw = p.H * p.W;
+            b0 = m0 / hw;
+            h0 = (m0 - b0 * hw) / p.W;
+            w0 = m0 - b0 * hw - h0 * p.W;      // != 0 only for rows wider than a tile (W > 128: the tile is a 128-pixel row segment)
           }
-          if (++kc == kb_per_tap) { kc = 0; ++seg; }
+          int seg = kb0 / kb_per_tap, kc = kb0 - seg * kb_per_tap;
+          for (int kb = kb0; kb < kb1; ++kb) {
+            const int tap = seg % p.taps;            // activation geometry of this segment; the weight column offset is seg * C
+            const int ky = tap / 3, kx = tap - ky * 3;
+            {
+              mbar_wait(&empty_bar[stage], phase ^ 1);
+              uint8_t* sa = smem + (size_t)stage * lay.stage_bytes;
+              uint8_t* sb = sa + GEMM_A_STAGE_BYTES;
+              mbar_arrive_expect_tx(&full_bar[stage], tx_bytes);
+              if (p.taps == 9)
+                tma_load_4d(sa, &tmA, &full_bar[stage], kc * GEMM_BK, w0 + kx - 1, h0 + ky - 1, b0);
+              else
+                tma_load_4d(sa, &tmA, &full_bar[stage], kc * GEMM_BK, m0, 0, 0);
+              if constexpr (W4)
+                tma_load_2d(smem + lay.pack_off + (size_t)stage * p.BN * (GEMM_BK / 2), &tmB, &full_bar[stage],
+                            (seg * p.C + kc * GEMM_BK) / 2, n0);
+              else
+                tma_load_2d(sb, &tmB, &full_bar[stage], seg * p.C + kc * GEMM_BK, n0);
+              if (++stage == p.stages) { stage = 0; phase ^= 1; }
+            }
+            if (++kc == kb_per_tap) { kc = 0; ++seg; }
+          }
         }
       }
-    }
-  } else if (warp == 2 || warp == 3 || warp >= 4 + EPI_WARPS) {
-    // ===================== INT4 unpack (warps 2, 3 and the two warps behind the epilogue warps; W4 only) ==========
-    // 128 threads = 32 rows x 4 sixteen-byte pieces per pass.  A piece holds 32 codes (k = 32j .. 32j+31 of the
-    // k-block) and becomes two 16-byte chunks of the row in the 128B-swizzled s8 tile the MMA descriptor expects
-    // (chunk index XOR row&7, identical to what TMA SWIZZLE_128B writes on the unpacked path).
-    // Nibble order (ops.pack_int4): byte j of a 4-byte word holds code k0+j in its low and code k0+4+j in its high nibble,
-    // so the masked word IS four consecutive codes - no byte permutation.  code - zp per byte without borrows:
-    // (code + (0x80 - zp)) ^ 0x80, the constant 0x80808080 - zp*0x01010101 kept per row.  7 integer instructions per 8
-    // codes (round 1: 11, on two warps: 1.7 k cycles per k-block against 0.9 k for the main loop).
-    if constexpr (W4) {
-      const int t = warp < 4 ? (int)threadIdx.x - 64 : (int)threadIdx.x - (4 + EPI_WARPS) * 32 + 64;   // 0..127
-      const int r32 = t >> 2, piece = t & 3;
-      int stage = 0;
-      uint32_t phase = 0;
-      for (int item = blockIdx.x; item < num_tiles; item += gridDim.x) {
-        const int tile = item / splits;
-        const int kb0 = (item - tile * splits) * kb_slice;
-        const int num_kb = min(num_kb_all, kb0 + kb_slice) - kb0;
-        const int tn = tile % p.tiles_n;
-        const int n0 = tn * p.BN;
-        uint32_t kz[8];       // 0x80808080 - zero point replicated into 4 bytes, rows r32 + 32*i
-#pragma unroll
-        for (int i = 0; i < 8; ++i) {
-          const int n = n0 + r32 + 32 * i;
-          kz[i] = 0x80808080u - ((r32 + 32 * i < p.BN && n < p.N) ? 0x01010101u * (uint32_t)(uint8_t)__ldg(p.wzero + n) : 0u);
-        }
-        for (int kb = 0; kb < num_kb; ++kb) {
-          mbar_wait(&full_bar[stage], phase);
-          const uint8_t* sp = smem + lay.pack_off + (size_t)stage * p.BN * (GEMM_BK / 2);
-          uint8_t* sb = smem + (size_t)stage * lay.stage_bytes + GEMM_A_STAGE_BYTES;
+    } else if (W4 && warp != 1) {
+      // ===================== INT4 unpack (warps 2, 3 and the two warps behind the consumer warps; W4 only) ==========
+      // 128 threads = 32 rows x 4 sixteen-byte pieces per pass.  A piece holds 32 codes (k = 32j .. 32j+31 of the
+      // k-block) and becomes two 16-byte chunks of the row in the 128B-swizzled s8 tile the MMA descriptor expects
+      // (chunk index XOR row&7, identical to what TMA SWIZZLE_128B writes on the unpacked path).
+      // Nibble order (ops.pack_int4): byte j of a 4-byte word holds code k0+j in its low and code k0+4+j in its high nibble,
+      // so the masked word IS four consecutive codes - no byte permutation.  code - zp per byte without borrows:
+      // (code + (0x80 - zp)) ^ 0x80, the constant 0x80808080 - zp*0x01010101 kept per row.  7 integer instructions per 8
+      // codes (round 1: 11, on two warps: 1.7 k cycles per k-block against 0.9 k for the main loop).
+      if constexpr (W4) {
+        const int t = warp < 4 ? (int)threadIdx.x - 64 : (int)threadIdx.x - GEMM_W4_WARP0 * 32 + 64;   // 0..127
+        const int r32 = t >> 2, piece = t & 3;
+        int stage = 0;
+        uint32_t phase = 0;
+        for (int item = blockIdx.x; item < num_tiles; item += gridDim.x) {
+          const int tile = item / splits;
+          const int kb0 = (item - tile * splits) * kb_slice;
+          const int num_kb = min(num_kb_all, kb0 + kb_slice) - kb0;
+          const int tn = tile % p.tiles_n;
+          const int n0 = tn * p.BN;
+          uint32_t kz[8];       // 0x80808080 - zero point replicated into 4 bytes, rows r32 + 32*i
 #pragma unroll
           for (int i = 0; i < 8; ++i) {
-            const int row = r32 + 32 * i;
-            if (row < p.BN) {
-              const uint4 w = *reinterpret_cast<const uint4*>(sp + row * (GEMM_BK / 2) + piece * 16);
-              const uint32_t in[4] = {w.x, w.y, w.z, w.w};
-              uint32_t o[8];
-#pragma unroll
-              for (int q = 0; q < 4; ++q) {
-                o[2 * q] = ((in[q] & 0x0F0F0F0Fu) + kz[i]) ^ 0x80808080u;             // k = 8q+0..3
-                o[2 * q + 1] = (((in[q] >> 4) & 0x0F0F0F0Fu) + kz[i]) ^ 0x80808080u;  // k = 8q+4..7
-              }
-              uint8_t* dst = sb + row * GEMM_BK;
-              *reinterpret_cast<uint4*>(dst + (((2 * piece) ^ (row & 7)) << 4)) = make_uint4(o[0], o[1], o[2], o[3]);
-              *reinterpret_cast<uint4*>(dst + (((2 * piece + 1) ^ (row & 7)) << 4)) = make_uint4(o[4], o[5], o[6], o[7]);
-            }
+            const int n = n0 + r32 + 32 * i;
+            kz[i] = 0x80808080u - ((r32 + 32 * i < p.BN && n < p.N) ? 0x01010101u * (uint32_t)(uint8_t)__ldg(p.wzero + n) : 0u);
           }
-          fence_proxy_async();     // generic-proxy smem writes -> visible to the tensor core (async proxy)
-          __syncwarp();
-          if (lane == 0) mbar_arrive(&ready_bar[stage]);
-          if (++stage == p.stages) { stage = 0; phase ^= 1; }
+          for (int kb = 0; kb < num_kb; ++kb) {
+            mbar_wait(&full_bar[stage], phase);
+            const uint8_t* sp = smem + lay.pack_off + (size_t)stage * p.BN * (GEMM_BK / 2);
+            uint8_t* sb = smem + (size_t)stage * lay.stage_bytes + GEMM_A_STAGE_BYTES;
+#pragma unroll
+            for (int i = 0; i < 8; ++i) {
+              const int row = r32 + 32 * i;
+              if (row < p.BN) {
+                const uint4 w = *reinterpret_cast<const uint4*>(sp + row * (GEMM_BK / 2) + piece * 16);
+                const uint32_t in[4] = {w.x, w.y, w.z, w.w};
+                uint32_t o[8];
+#pragma unroll
+                for (int q = 0; q < 4; ++q) {
+                  o[2 * q] = ((in[q] & 0x0F0F0F0Fu) + kz[i]) ^ 0x80808080u;             // k = 8q+0..3
+                  o[2 * q + 1] = (((in[q] >> 4) & 0x0F0F0F0Fu) + kz[i]) ^ 0x80808080u;  // k = 8q+4..7
+                }
+                uint8_t* dst = sb + row * GEMM_BK;
+                *reinterpret_cast<uint4*>(dst + (((2 * piece) ^ (row & 7)) << 4)) = make_uint4(o[0], o[1], o[2], o[3]);
+                *reinterpret_cast<uint4*>(dst + (((2 * piece + 1) ^ (row & 7)) << 4)) = make_uint4(o[4], o[5], o[6], o[7]);
+              }
+            }
+            fence_proxy_async();     // generic-proxy smem writes -> visible to the tensor core (async proxy)
+            __syncwarp();
+            if (lane == 0) mbar_arrive(&ready_bar[stage]);
+            if (++stage == p.stages) { stage = 0; phase ^= 1; }
+          }
         }
       }
     }
-  } else if (warp >= 4 && warp < 4 + EPI_WARPS) {
-    // ===================== consumers: wgmma main loop, then the epilogue =====================
+  } else {
+    // ===================== consumers (warps 4-11): wgmma main loop -> accumulator tile; epilogue warps =====================
     // The accumulators leave the registers into the shared-memory accumulator tile (32 x 32 int32 chunks, 128 B rows,
     // 16 B units XOR-swizzled by row&7: conflict-free both ways); the epilogue reads each chunk in the transposed
     // mapping: 8 lanes x 16 B = one full 128 B line per row, 4 rows per instruction, per-column parameters loaded once
@@ -587,120 +638,77 @@ gemm_i8_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     const int cw = warp - 4;            // consumer warp 0..7
     const int wg = cw >> 2;             // its warpgroup: accumulator rows [64 wg, 64 wg + 64)
     const bool wg_leader = (threadIdx.x & 127) == 0;
-    const int q = cw & 3;               // epilogue: row quarter [32q, 32q + 32) of the tile
-    const int half = cw >> 2;           // which of the two warps sharing this row quarter
     const int nch = (p.BN + 31) >> 5;   // 32-column chunks per row quarter of the accumulator tile
     uint8_t* const acc_tile = smem + lay.stage_off;
-    const uint8_t* stg = acc_tile;
     constexpr bool BF16 = MODE >= 0 && (MODE & EPI_BF16) != 0;
     using AccT = typename std::conditional<BF16, float, uint32_t>::type;
     int stage = 0;
     uint32_t phase = 0;
-    const int rsub = lane >> 3;   // row within a group of 4
-    const int cq = lane & 7;      // column quad within the 32-column chunk
-    constexpr bool QPRE = gemm_qpre(MODE);
-    const QuantK qk = QPRE ? make_quantk_pre(p.q_delta, p.q_lo, p.q_hi) : make_quantk(p.q_delta, p.q_zp, p.q_lo, p.q_hi);
-    const float* const ep_scale = QPRE ? p.scale_q : p.scale;      // per-column epilogue constants of this mode
-    const float* const ep_bias = QPRE ? p.bias_q : p.bias;
-    const bool conv = MODE < 0 ? (p.taps == 9) : ((MODE & EPI_CONV) != 0);
-    // ---- residual ring (RES_TMA): work items of this warp = (tile, chunk) in processing order; `pf_*` is the prefetch
-    // cursor, GEMM_RES_NBUF - 1 items ahead of the item being finalised
-    uint8_t* rring = smem + lay.res_off + (warp - 4) * (GEMM_RES_NBUF * 4096);
-    uint64_t* rbar = res_bar + (warp - 4) * GEMM_RES_NBUF;
-    int pf_tile = blockIdx.x, pf_c = half * 32, pf_buf = 0;
-    int rd_buf = 0;
-    uint32_t rd_phase = 0;
-    auto res_issue = [&]() {          // issue the load of the cursor's item (if any) and advance the cursor
-      if (pf_tile >= num_tiles) return;
-      if (lane == 0) {
-        const int ptm = pf_tile / p.tiles_n, ptn = pf_tile - ptm * p.tiles_n;
-        mbar_arrive_expect_tx(&rbar[pf_buf], 4096u);
-        tma_load_2d(rring + pf_buf * 4096, &tmR, &rbar[pf_buf], (ptn * p.BN + pf_c) * 4, ptm * GEMM_BM + q * 32);
-      }
-      if (++pf_buf == GEMM_RES_NBUF) pf_buf = 0;
-      pf_c += CSTEP;
-      if (pf_c >= p.BN) { pf_c = half * 32; pf_tile += gridDim.x; }
-    };
-    if constexpr (RES_TMA) {
-      if (half * 32 >= p.BN) pf_tile = num_tiles;      // this warp owns no chunk (BN narrower than its first column)
-#pragma unroll 1
-      for (int i = 0; i < GEMM_RES_NBUF - 1; ++i) res_issue();
-    }
-    for (int item = blockIdx.x; item < num_tiles; item += gridDim.x) {
+
+    // ---- consumer: main loop of one work item over its k-blocks [kb0, kb1); a stage returns to the producer once the
+    // MMAs reading it are complete (one k-block of MMAs stays in flight).  Then the accumulators go to the accumulator
+    // tile once `before_dump()` returns (the previous item's epilogue has read it), or - split-K partials - straight from
+    // the registers to the workspace.  The accumulators live in this scope only.
+    auto consume = [&](const int item, auto&& before_dump) {
       const int tile = item / splits;
       const int zsplit = item - tile * splits;
-      const int tm = tile / p.tiles_n;
-      const int tn = tile - tm * p.tiles_n;
-      const int n_base = tn * p.BN;
-      const int m_warp = tm * GEMM_BM + q * 32;
-      const bool transposed = (MODE < 0) && p.out_q_transposed;
-      constexpr bool kTrans = MODE >= 0 && (MODE & EPI_TRANS) != 0;
-      int cls8[8], img8[8];
-      if (!transposed && !kTrans) {
+      AccT accr[NS][32];
 #pragma unroll
-        for (int it = 0; it < 8; ++it) gemm_row_meta(p, m_warp + it * 4 + rsub, cls8[it], img8[it]);
-      }
-      // ---- main loop: k-blocks [kb0, kb1) of this work item; a stage returns to the producer once the MMAs reading it
-      // are complete (one k-block of MMAs stays in flight).  The accumulators live in this scope only: dead during the
-      // epilogue, whose registers they would otherwise take.
-      {
-        AccT accr[NS][32];
+      for (int s = 0; s < NS; ++s)
+#pragma unroll
+        for (int i = 0; i < 32; ++i) accr[s][i] = 0;
+      const int kb0 = zsplit * kb_slice;
+      const int kb1 = min(num_kb_all, kb0 + kb_slice);
+      int prev_stage = -1;
+      // the N-tile width and the operand signedness are selected once per work item; each configuration's k-loop is
+      // its own straight-line wgmma sequence
+      auto mainloop = [&](auto cfg) {
+        using Cfg = decltype(cfg);
+        for (int kb = kb0; kb < kb1; ++kb) {
+          mbar_wait(&full_bar[stage], phase);
+          if constexpr (W4) mbar_wait(&ready_bar[stage], phase);   // ... and the B tile has been unpacked
+          wgmma_fence();
+          const uint32_t sa = smem_u32(smem + (size_t)stage * lay.stage_bytes);
+          const uint64_t da = make_smem_desc_sw128(sa + (uint32_t)(wg * 64 * GEMM_BK));
+          const uint64_t db = make_smem_desc_sw128(sa + GEMM_A_STAGE_BYTES);
+          gemm_wgmma_kblock<BF16, Cfg::SIGNED, Cfg::NF, Cfg::TAIL>(accr, da, db, kb > kb0 ? 1u : 0u);
+          wgmma_commit();
+          wgmma_wait<1>();
+          if (prev_stage >= 0 && wg_leader) mbar_arrive(&empty_bar[prev_stage]);
+          prev_stage = stage;
+          if (++stage == p.stages) { stage = 0; phase ^= 1; }
+        }
+        wgmma_wait<0>();
+      };
+      if constexpr (BF16) gemm_dispatch_bn<NS, true>(p.BN, mainloop);
+      else if (p.a_signed) gemm_dispatch_bn<NS, true>(p.BN, mainloop);
+      else gemm_dispatch_bn<NS, false>(p.BN, mainloop);
+#pragma unroll
+      for (int s = 0; s < NS; ++s) wgmma_fence_regs(accr[s]);
+      if (prev_stage >= 0 && wg_leader) mbar_arrive(&empty_bar[prev_stage]);
+      const int r0 = 64 * wg + 16 * (cw & 3) + (lane >> 2);
+      if constexpr (SPLITK) {
+        // raw accumulators of this K slice -> ws[zsplit][M][N] straight from the registers (host: N % 4 == 0); a warp
+        // store covers 8 rows x 32 contiguous bytes
+        const int tm = tile / p.tiles_n;
+        const int n_base = (tile - tm * p.tiles_n) * p.BN;
+        int32_t* wz = p.ws + (long long)zsplit * p.M * p.N;
 #pragma unroll
         for (int s = 0; s < NS; ++s)
 #pragma unroll
-          for (int i = 0; i < 32; ++i) accr[s][i] = 0;
-        const int kb0 = zsplit * kb_slice;
-        const int kb1 = min(num_kb_all, kb0 + kb_slice);
-        int prev_stage = -1;
-        // the N-tile width and the operand signedness are selected once per work item; each configuration's k-loop is
-        // its own straight-line wgmma sequence
-        auto mainloop = [&](auto cfg) {
-          using Cfg = decltype(cfg);
-          for (int kb = kb0; kb < kb1; ++kb) {
-            mbar_wait(&full_bar[stage], phase);
-            if constexpr (W4) mbar_wait(&ready_bar[stage], phase);   // ... and the B tile has been unpacked
-            wgmma_fence();
-            const uint32_t sa = smem_u32(smem + (size_t)stage * lay.stage_bytes);
-            const uint64_t da = make_smem_desc_sw128(sa + (uint32_t)(wg * 64 * GEMM_BK));
-            const uint64_t db = make_smem_desc_sw128(sa + GEMM_A_STAGE_BYTES);
-            gemm_wgmma_kblock<BF16, Cfg::SIGNED, Cfg::NF, Cfg::TAIL>(accr, da, db, kb > kb0 ? 1u : 0u);
-            wgmma_commit();
-            wgmma_wait<1>();
-            if (prev_stage >= 0 && wg_leader) mbar_arrive(&empty_bar[prev_stage]);
-            prev_stage = stage;
-            if (++stage == p.stages) { stage = 0; phase ^= 1; }
-          }
-          wgmma_wait<0>();
-        };
-        if constexpr (BF16) gemm_dispatch_bn<NS, true>(p.BN, mainloop);
-        else if (p.a_signed) gemm_dispatch_bn<NS, true>(p.BN, mainloop);
-        else gemm_dispatch_bn<NS, false>(p.BN, mainloop);
+          for (int j = 0; j < 8; ++j) {
+            const int n = n_base + 64 * s + 8 * j + 2 * (lane & 3);
+            if (64 * s + 8 * j < p.BN && n < p.N) {
 #pragma unroll
-        for (int s = 0; s < NS; ++s) wgmma_fence_regs(accr[s]);
-        if (prev_stage >= 0 && wg_leader) mbar_arrive(&empty_bar[prev_stage]);
-        const int r0 = 64 * wg + 16 * (cw & 3) + (lane >> 2);
-        if constexpr (SPLITK) {
-          // raw accumulators of this K slice -> ws[zsplit][M][N] straight from the registers (host: N % 4 == 0); a warp
-          // store covers 8 rows x 32 contiguous bytes
-          int32_t* wz = p.ws + (long long)zsplit * p.M * p.N;
-#pragma unroll
-          for (int s = 0; s < NS; ++s)
-#pragma unroll
-            for (int j = 0; j < 8; ++j) {
-              const int n = n_base + 64 * s + 8 * j + 2 * (lane & 3);
-              if (64 * s + 8 * j < p.BN && n < p.N) {
-#pragma unroll
-                for (int h = 0; h < 2; ++h) {
-                  const int m = tm * GEMM_BM + r0 + 8 * h;
-                  if (m < p.M)
-                    *reinterpret_cast<uint2*>(wz + (long long)m * p.N + n) = make_uint2(accr[s][4 * j + 2 * h], accr[s][4 * j + 2 * h + 1]);
-                }
+              for (int h = 0; h < 2; ++h) {
+                const int m = tm * GEMM_BM + r0 + 8 * h;
+                if (m < p.M)
+                  *reinterpret_cast<uint2*>(wz + (long long)m * p.N + n) = make_uint2(accr[s][4 * j + 2 * h], accr[s][4 * j + 2 * h + 1]);
               }
             }
-          continue;
-        }
-        // ---- accumulators -> accumulator tile (after every consumer warp has finished reading the previous tile's)
-        named_bar_sync(1, EPI_WARPS * 32);
+          }
+      } else {
+        before_dump();
 #pragma unroll
         for (int s = 0; s < NS; ++s)
 #pragma unroll
@@ -720,212 +728,313 @@ gemm_i8_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
             }
           }
       }
-      named_bar_sync(1, EPI_WARPS * 32);
-      if constexpr (kTrans) {
-        // V^T code output [img][n][token'] (token' = att_vt_perm order inside each group of 16).  The warp's
-        // 32 tokens x 32 channels go through the staging tile; each lane then owns ONE channel and emits whole
-        // 16-token groups as 16 B stores (the thread-per-row form below needs 32 byte stores per lane and chunk).
-        // Host guarantees rows_per_batch % 32 == 0 (a warp never straddles images), ldq % 16 == 0.
-        const int img = m_warp / p.rows_per_batch;
-        const int tok0 = m_warp - img * p.rows_per_batch;
-        for (int c = half * 32; c < p.BN; c += CSTEP) {
-          const int ncols = (p.BN - c) >= 32 ? 32 : 16;
-          stg = acc_tile + (q * nch + (c >> 5)) * GEMM_EPI_TILE_BYTES;
-          const int col = ncols == 32 ? lane : (lane & 15);
-          const int n = n_base + c + col;
-          if (m_warp < p.M && n < p.N) {
-            const float sc1 = __ldg(ep_scale + n);
-            const float bi1 = ep_bias ? __ldg(ep_bias + n) : 0.f;
-            int cr = 0;
-            if constexpr ((MODE & EPI_CORR) != 0) cr = __ldg(p.corr + n);
-            int8_t* o = p.out_q + ((long long)img * p.N + n) * p.ldq + tok0;
-            const uint8_t* src = stg + (col & 3) * 4;
-            const int cj = col >> 2;
-            const int g0 = ncols == 32 ? 0 : (lane >> 4), g1 = ncols == 32 ? 2 : g0 + 1;
-            for (int g = g0; g < g1; ++g) {
-              uint32_t w4[4];
-#pragma unroll
-              for (int k = 0; k < 16; ++k) {
-                const int r7 = (((k >> 1) & 1) << 3) | (((k >> 2) & 3) << 1) | (k & 1);   // token of byte k
-                const int a = *reinterpret_cast<const int*>(src + (g * 16 + r7) * 128 + ((cj ^ (r7 & 7)) << 4));
-                const uint32_t qv = QPRE ? (quant_bits_pre(fmaf((float)(a - cr), sc1, bi1), qk) & 0xFFu)
-                                         : quant_code((float)(a - cr) * sc1 + bi1, qk);
-                w4[k >> 2] = (k & 3) ? (w4[k >> 2] | (qv << (8 * (k & 3)))) : qv;
-              }
-              *reinterpret_cast<uint4*>(o + g * 16) = make_uint4(w4[0], w4[1], w4[2], w4[3]);
-            }
-          }
-          __syncwarp();
+    };
+
+    // ---- epilogue warp `ew` (0 .. EPI_WARPS - 1): finalises rows [32q, 32q + 32) of each work item's tile, 32-column
+    // chunks half * 32, half * 32 + CSTEP, ...  `acquire(item)` returns once the item's accumulators are in the tile,
+    // `release()` follows the warp's last read of it.
+    auto epilogue = [&](const int ew, auto&& acquire, auto&& release) {
+      const int q = ew & 3;               // row quarter [32q, 32q + 32) of the tile
+      const int half = ew >> 2;           // which of the EPI_WARPS / 4 warps sharing this row quarter
+      const int rsub = lane >> 3;   // row within a group of 4
+      [[maybe_unused]] const int cq = lane & 7;      // column quad within the 32-column chunk
+      constexpr bool QPRE = gemm_qpre(MODE);
+      const QuantK qk = QPRE ? make_quantk_pre(p.q_delta, p.q_lo, p.q_hi) : make_quantk(p.q_delta, p.q_zp, p.q_lo, p.q_hi);
+      const float* const ep_scale = QPRE ? p.scale_q : p.scale;      // per-column epilogue constants of this mode
+      const float* const ep_bias = QPRE ? p.bias_q : p.bias;
+      [[maybe_unused]] const bool conv = MODE < 0 ? (p.taps == 9) : ((MODE & EPI_CONV) != 0);
+      // ---- residual ring (RES_TMA): work items of this warp = (tile, chunk) in processing order; `pf_*` is the prefetch
+      // cursor, GEMM_RES_NBUF - 1 items ahead of the item being finalised
+      uint8_t* rring = smem + lay.res_off + ew * (GEMM_RES_NBUF * 4096);
+      uint64_t* rbar = res_bar + ew * GEMM_RES_NBUF;
+      int pf_tile = blockIdx.x, pf_c = half * 32, pf_buf = 0;
+      [[maybe_unused]] int rd_buf = 0;
+      [[maybe_unused]] uint32_t rd_phase = 0;
+      auto res_issue = [&]() {          // issue the load of the cursor's item (if any) and advance the cursor
+        if (pf_tile >= num_tiles) return;
+        if (lane == 0) {
+          const int ptm = pf_tile / p.tiles_n, ptn = pf_tile - ptm * p.tiles_n;
+          mbar_arrive_expect_tx(&rbar[pf_buf], 4096u);
+          tma_load_2d(rring + pf_buf * 4096, &tmR, &rbar[pf_buf], (ptn * p.BN + pf_c) * 4, ptm * GEMM_BM + q * 32);
         }
-      } else if constexpr (MODE >= 0 && (MODE & EPI_GEGLU) != 0) {
-        // GEGLU projection (ldm/modules/attention.py:42-44) fused with the consumer's quantizer: a 32-column chunk
-        // holds 4 x (4 x-features | 4 gate-features); lane -> (row group of 8, pair); 4 iterations cover 32 rows.
-        const int r8 = lane >> 2, pq = lane & 3;
-        for (int c = half * 32; c < p.BN; c += CSTEP) {
-          stg = acc_tile + (q * nch + (c >> 5)) * GEMM_EPI_TILE_BYTES;
-          const int nx = n_base + c + 8 * pq;          // 4 x columns, then 4 gate columns
-          if (nx < p.N) {
-            const float4 sx = __ldg(reinterpret_cast<const float4*>(p.scale + nx));
-            const float4 sg = __ldg(reinterpret_cast<const float4*>(p.scale + nx + 4));
-            float4 bx = make_float4(0.f, 0.f, 0.f, 0.f), bg = bx;
-            if (p.bias) {
-              bx = __ldg(reinterpret_cast<const float4*>(p.bias + nx));
-              bg = __ldg(reinterpret_cast<const float4*>(p.bias + nx + 4));
-            }
-            int4 cx = make_int4(0, 0, 0, 0), cg = cx;
-            if constexpr ((MODE & EPI_CORR) != 0) {
-              cx = __ldg(reinterpret_cast<const int4*>(p.corr + nx));
-              cg = __ldg(reinterpret_cast<const int4*>(p.corr + nx + 4));
-            }
-#pragma unroll
-            for (int it = 0; it < 4; ++it) {
-              const int row = it * 8 + r8;
-              const int m = m_warp + row;
-              if (m < p.M) {
-                const uint4 ax = *reinterpret_cast<const uint4*>(stg + row * 128 + (((2 * pq) ^ (row & 7)) << 4));
-                const uint4 ag = *reinterpret_cast<const uint4*>(stg + row * 128 + (((2 * pq + 1) ^ (row & 7)) << 4));
-                const float x0 = (float)((int)ax.x - cx.x) * sx.x + bx.x, g0 = (float)((int)ag.x - cg.x) * sg.x + bg.x;
-                const float x1 = (float)((int)ax.y - cx.y) * sx.y + bx.y, g1 = (float)((int)ag.y - cg.y) * sg.y + bg.y;
-                const float x2 = (float)((int)ax.z - cx.z) * sx.z + bx.z, g2 = (float)((int)ag.z - cg.z) * sg.z + bg.z;
-                const float x3 = (float)((int)ax.w - cx.w) * sx.w + bx.w, g3 = (float)((int)ag.w - cg.w) * sg.w + bg.w;
-                const uint32_t code = quant_code_fast(x0 * gelu_fast(g0), qk) | (quant_code_fast(x1 * gelu_fast(g1), qk) << 8) |
-                                      (quant_code_fast(x2 * gelu_fast(g2), qk) << 16) | (quant_code_fast(x3 * gelu_fast(g3), qk) << 24);
-                *reinterpret_cast<uint32_t*>(p.out_q + (long long)m * p.ldq + (nx >> 1)) = code;
-              }
-            }
-          }
-          __syncwarp();
-        }
-      } else if (transposed) {
-        const int m = m_warp + lane;
-        int cls, img;
-        gemm_row_meta(p, m, cls, img);
-        for (int c = half * 32; c < p.BN; c += CSTEP) {
-          if (p.BN - c >= 32) {
-            uint32_t v[32];
-            gemm_acc_row(acc_tile + (q * nch + (c >> 5)) * GEMM_EPI_TILE_BYTES, lane, v);
-            if (m < p.M && n_base + c < p.N) gemm_epilogue_rowwise<32>(p, qk, v, m, n_base + c, cls, img);
-          } else {
-            uint32_t v[16];
-            gemm_acc_row(acc_tile + (q * nch + (c >> 5)) * GEMM_EPI_TILE_BYTES, lane, v);
-            if (m < p.M && n_base + c < p.N) gemm_epilogue_rowwise<16>(p, qk, v, m, n_base + c, cls, img);
-          }
-        }
-      } else {
-        for (int c = half * 32; c < p.BN; c += CSTEP) {
-          const int ncols = (p.BN - c) >= 32 ? 32 : 16;
-          stg = acc_tile + (q * nch + (c >> 5)) * GEMM_EPI_TILE_BYTES;
-          const uint8_t* rbuf = nullptr;
-          if constexpr (RES_TMA) {
-            res_issue();                              // keep GEMM_RES_NBUF - 1 loads in flight
-            mbar_wait(&rbar[rd_buf], rd_phase);       // this item's residual sub-tile (32 rows x 128 B, 128B-swizzled)
-            rbuf = rring + rd_buf * 4096;
-          }
-          const int n = n_base + c + cq * 4;
-          const bool col_ok = cq * 4 < ncols && n < p.N;
-          const unsigned cmask = __ballot_sync(0xffffffffu, col_ok);   // lanes ^8 / ^16 share cq: partners are always both in or out
-          if (col_ok) {
-            float sc[4], bi[4];
-            int4 corr4 = make_int4(0, 0, 0, 0);
-            if (MODE >= 0 || n + 3 < p.N) {
-              const float4 s4 = *reinterpret_cast<const float4*>(ep_scale + n);
-              sc[0] = s4.x; sc[1] = s4.y; sc[2] = s4.z; sc[3] = s4.w;
-              if (ep_bias) {
-                const float4 b4 = *reinterpret_cast<const float4*>(ep_bias + n);
-                bi[0] = b4.x; bi[1] = b4.y; bi[2] = b4.z; bi[3] = b4.w;
-              } else {
-                bi[0] = bi[1] = bi[2] = bi[3] = 0.f;
-              }
-              if (p.corr && !conv) corr4 = *reinterpret_cast<const int4*>(p.corr + n);
-            } else {
-              int cc[4] = {0, 0, 0, 0};
-#pragma unroll
-              for (int j = 0; j < 4; ++j) {
-                const bool ok = n + j < p.N;
-                sc[j] = ok ? __ldg(p.scale + n + j) : 0.f;
-                bi[j] = (ok && p.bias) ? __ldg(p.bias + n + j) : 0.f;
-                cc[j] = (ok && p.corr && !conv) ? __ldg(p.corr + n + j) : 0;
-              }
-              corr4 = make_int4(cc[0], cc[1], cc[2], cc[3]);
-            }
-            int nq = n;   // column of the code output (per-head padded layout: attention Q/K operands)
-            if (p.oq_d > 0) { const int hq = n / p.oq_d; nq = hq * p.oq_pitch + (n - hq * p.oq_d); }
-            // Rows are finalised four at a time with everything they need from global memory (residual, conv
-            // border-class correction) fetched up front, and - on the full-tile path - without any per-row
-            // branch: the `m < M` tests split the unrolled loop into basic blocks, and with two epilogue warps
-            // per scheduler the resulting dependent-issue chains (stall_wait) bounded the small-K GEMMs.
-            const long long mrow = m_warp + rsub;
-            float* of0 = p.out ? p.out + mrow * p.ldo + n : nullptr;
-            const int oq_es = p.oq_f16 ? 2 : 1;      // bytes per emitted code
-            int8_t* oq0 = p.out_q ? p.out_q + (mrow * p.ldq + nq) * oq_es : nullptr;
-            const float* res0 = p.residual ? p.residual + mrow * p.ldr + n : nullptr;
-            const long long of_step = 4 * p.ldo, oq_step = 4 * p.ldq * oq_es, res_step = 4 * p.ldr;
-            float gsum[4] = {0.f, 0.f, 0.f, 0.f}, gsq[4] = {0.f, 0.f, 0.f, 0.f};
-            auto rows = [&](auto full_tag) {
-              constexpr bool FULL = decltype(full_tag)::value;
-#pragma unroll
-              for (int h4 = 0; h4 < 8; h4 += 4) {
-                float4 rpre[4];
-                int4 cpre[4];
-#pragma unroll
-                for (int i = 0; i < 4; ++i) {
-                  const int it = h4 + i;
-                  [[maybe_unused]] const int m = m_warp + it * 4 + rsub;
-                  rpre[i] = make_float4(0.f, 0.f, 0.f, 0.f);
-                  cpre[i] = corr4;
-                  if constexpr (RES_TMA) {
-                    const int row = it * 4 + rsub;    // rows beyond M were zero-filled by the TMA unit
-                    rpre[i] = *reinterpret_cast<const float4*>(rbuf + row * 128 + ((cq ^ (row & 7)) << 4));
-                  } else if constexpr (MODE >= 0 && (MODE & EPI_RESIDUAL) != 0) {
-                    if (FULL || m < p.M) rpre[i] = *reinterpret_cast<const float4*>(res0 + it * res_step);
-                  }
-                  if constexpr (MODE >= 0 && (MODE & EPI_CORR) != 0 && (MODE & EPI_CONV) != 0)
-                    cpre[i] = __ldg(reinterpret_cast<const int4*>(p.corr + (long long)cls8[it] * p.N + n));
-                }
-#pragma unroll
-                for (int i = 0; i < 4; ++i) {
-                  const int it = h4 + i;
-                  const int row = it * 4 + rsub;
-                  const int m = m_warp + row;
-                  if (FULL || m < p.M) {
-                    const uint4 a4 = *reinterpret_cast<const uint4*>(stg + row * 128 + ((cq ^ (row & 7)) << 4));
-                    gemm_finalise4<MODE>(p, qk, conv, a4, sc, bi, cpre[i], rpre[i], of0 + it * of_step, oq0 + it * oq_step,
-                                         res0 + it * res_step, n, cls8[it], img8[it], gsum, gsq);
-                  }
-                }
-              }
-            };
-            if (m_warp + 32 <= p.M) rows(std::true_type{}); else rows(std::false_type{});
-            if ((MODE < 0 || (MODE & EPI_OUT_F32) != 0) && p.gn_stats != nullptr) {
-              // this thread holds 8 of the slab's 32 rows for 4 columns: add the other three row groups (lanes ^ 8, ^ 16),
-              // lanes 0-7 then own the slab's column sums for the chunk's 32 columns
-#pragma unroll
-              for (int j = 0; j < 4; ++j) {
-                gsum[j] += __shfl_xor_sync(cmask, gsum[j], 8);
-                gsq[j] += __shfl_xor_sync(cmask, gsq[j], 8);
-                gsum[j] += __shfl_xor_sync(cmask, gsum[j], 16);
-                gsq[j] += __shfl_xor_sync(cmask, gsq[j], 16);
-              }
-              if (rsub == 0) {
-                float2* st = p.gn_stats + (long long)(m_warp >> 5) * p.ld_stats + n;
-                if (MODE >= 0 || n + 3 < p.N) {
-                  *reinterpret_cast<float4*>(st) = make_float4(gsum[0], gsq[0], gsum[1], gsq[1]);
-                  *reinterpret_cast<float4*>(st + 2) = make_float4(gsum[2], gsq[2], gsum[3], gsq[3]);
-                } else {
-#pragma unroll
-                  for (int j = 0; j < 4; ++j)
-                    if (n + j < p.N) st[j] = make_float2(gsum[j], gsq[j]);
-                }
-              }
-            }
-          }
-          if constexpr (RES_TMA) {
-            fence_proxy_async();      // this buffer's generic-proxy reads are ordered before the TMA write that reuses it
-            if (++rd_buf == GEMM_RES_NBUF) { rd_buf = 0; rd_phase ^= 1; }
-          }
-          __syncwarp();
-        }
+        if (++pf_buf == GEMM_RES_NBUF) pf_buf = 0;
+        pf_c += CSTEP;
+        if (pf_c >= p.BN) { pf_c = half * 32; pf_tile += gridDim.x; }
+      };
+      if constexpr (RES_TMA) {
+        if (half * 32 >= p.BN) pf_tile = num_tiles;      // this warp owns no chunk (BN narrower than its first column)
+#pragma unroll 1
+        for (int i = 0; i < GEMM_RES_NBUF - 1; ++i) res_issue();
       }
+      for (int item = blockIdx.x; item < num_tiles; item += gridDim.x) {
+        const int tile = item / splits;
+        const int tm = tile / p.tiles_n;
+        const int tn = tile - tm * p.tiles_n;
+        const int n_base = tn * p.BN;
+        const int m_warp = tm * GEMM_BM + q * 32;
+        const bool transposed = (MODE < 0) && p.out_q_transposed;
+        constexpr bool kTrans = MODE >= 0 && (MODE & EPI_TRANS) != 0;
+        int cls8[8], img8[8];
+        if (!transposed && !kTrans) {
+#pragma unroll
+          for (int it = 0; it < 8; ++it) gemm_row_meta(p, m_warp + it * 4 + rsub, cls8[it], img8[it]);
+        }
+        acquire(item);
+        if constexpr (kTrans) {
+          // V^T code output [img][n][token'] (token' = att_vt_perm order inside each group of 16).  The warp's
+          // 32 tokens x 32 channels go through the staging tile; each lane then owns ONE channel and emits whole
+          // 16-token groups as 16 B stores (the thread-per-row form below needs 32 byte stores per lane and chunk).
+          // Host guarantees rows_per_batch % 32 == 0 (a warp never straddles images), ldq % 16 == 0.
+          const int img = m_warp / p.rows_per_batch;
+          const int tok0 = m_warp - img * p.rows_per_batch;
+          for (int c = half * 32; c < p.BN; c += CSTEP) {
+            const int ncols = (p.BN - c) >= 32 ? 32 : 16;
+            const uint8_t* stg = acc_tile + (q * nch + (c >> 5)) * GEMM_EPI_TILE_BYTES;
+            const int col = ncols == 32 ? lane : (lane & 15);
+            const int n = n_base + c + col;
+            if (m_warp < p.M && n < p.N) {
+              const float sc1 = __ldg(ep_scale + n);
+              const float bi1 = ep_bias ? __ldg(ep_bias + n) : 0.f;
+              int cr = 0;
+              if constexpr ((MODE & EPI_CORR) != 0) cr = __ldg(p.corr + n);
+              int8_t* o = p.out_q + ((long long)img * p.N + n) * p.ldq + tok0;
+              const uint8_t* src = stg + (col & 3) * 4;
+              const int cj = col >> 2;
+              const int g0 = ncols == 32 ? 0 : (lane >> 4), g1 = ncols == 32 ? 2 : g0 + 1;
+              for (int g = g0; g < g1; ++g) {
+                uint32_t w4[4];
+#pragma unroll
+                for (int k = 0; k < 16; ++k) {
+                  const int r7 = (((k >> 1) & 1) << 3) | (((k >> 2) & 3) << 1) | (k & 1);   // token of byte k
+                  const int a = *reinterpret_cast<const int*>(src + (g * 16 + r7) * 128 + ((cj ^ (r7 & 7)) << 4));
+                  const uint32_t qv = QPRE ? (quant_bits_pre(fmaf((float)(a - cr), sc1, bi1), qk) & 0xFFu)
+                                           : quant_code((float)(a - cr) * sc1 + bi1, qk);
+                  w4[k >> 2] = (k & 3) ? (w4[k >> 2] | (qv << (8 * (k & 3)))) : qv;
+                }
+                *reinterpret_cast<uint4*>(o + g * 16) = make_uint4(w4[0], w4[1], w4[2], w4[3]);
+              }
+            }
+            __syncwarp();
+          }
+        } else if constexpr (MODE >= 0 && (MODE & EPI_GEGLU) != 0) {
+          // GEGLU projection (ldm/modules/attention.py:42-44) fused with the consumer's quantizer: a 32-column chunk
+          // holds 4 x (4 x-features | 4 gate-features); lane -> (row group of 8, pair); 4 iterations cover 32 rows.
+          const int r8 = lane >> 2, pq = lane & 3;
+          for (int c = half * 32; c < p.BN; c += CSTEP) {
+            const uint8_t* stg = acc_tile + (q * nch + (c >> 5)) * GEMM_EPI_TILE_BYTES;
+            const int nx = n_base + c + 8 * pq;          // 4 x columns, then 4 gate columns
+            if (nx < p.N) {
+              const float4 sx = __ldg(reinterpret_cast<const float4*>(p.scale + nx));
+              const float4 sg = __ldg(reinterpret_cast<const float4*>(p.scale + nx + 4));
+              float4 bx = make_float4(0.f, 0.f, 0.f, 0.f), bg = bx;
+              if (p.bias) {
+                bx = __ldg(reinterpret_cast<const float4*>(p.bias + nx));
+                bg = __ldg(reinterpret_cast<const float4*>(p.bias + nx + 4));
+              }
+              int4 cx = make_int4(0, 0, 0, 0), cg = cx;
+              if constexpr ((MODE & EPI_CORR) != 0) {
+                cx = __ldg(reinterpret_cast<const int4*>(p.corr + nx));
+                cg = __ldg(reinterpret_cast<const int4*>(p.corr + nx + 4));
+              }
+#pragma unroll
+              for (int it = 0; it < 4; ++it) {
+                const int row = it * 8 + r8;
+                const int m = m_warp + row;
+                if (m < p.M) {
+                  const uint4 ax = *reinterpret_cast<const uint4*>(stg + row * 128 + (((2 * pq) ^ (row & 7)) << 4));
+                  const uint4 ag = *reinterpret_cast<const uint4*>(stg + row * 128 + (((2 * pq + 1) ^ (row & 7)) << 4));
+                  const float x0 = (float)((int)ax.x - cx.x) * sx.x + bx.x, g0 = (float)((int)ag.x - cg.x) * sg.x + bg.x;
+                  const float x1 = (float)((int)ax.y - cx.y) * sx.y + bx.y, g1 = (float)((int)ag.y - cg.y) * sg.y + bg.y;
+                  const float x2 = (float)((int)ax.z - cx.z) * sx.z + bx.z, g2 = (float)((int)ag.z - cg.z) * sg.z + bg.z;
+                  const float x3 = (float)((int)ax.w - cx.w) * sx.w + bx.w, g3 = (float)((int)ag.w - cg.w) * sg.w + bg.w;
+                  const uint32_t code = quant_code_fast(x0 * gelu_fast(g0), qk) | (quant_code_fast(x1 * gelu_fast(g1), qk) << 8) |
+                                        (quant_code_fast(x2 * gelu_fast(g2), qk) << 16) | (quant_code_fast(x3 * gelu_fast(g3), qk) << 24);
+                  *reinterpret_cast<uint32_t*>(p.out_q + (long long)m * p.ldq + (nx >> 1)) = code;
+                }
+              }
+            }
+            __syncwarp();
+          }
+        } else if (transposed) {
+          const int m = m_warp + lane;
+          int cls, img;
+          gemm_row_meta(p, m, cls, img);
+          for (int c = half * 32; c < p.BN; c += CSTEP) {
+            if (p.BN - c >= 32) {
+              uint32_t v[32];
+              gemm_acc_row(acc_tile + (q * nch + (c >> 5)) * GEMM_EPI_TILE_BYTES, lane, v);
+              if (m < p.M && n_base + c < p.N) gemm_epilogue_rowwise<32>(p, qk, v, m, n_base + c, cls, img);
+            } else {
+              uint32_t v[16];
+              gemm_acc_row(acc_tile + (q * nch + (c >> 5)) * GEMM_EPI_TILE_BYTES, lane, v);
+              if (m < p.M && n_base + c < p.N) gemm_epilogue_rowwise<16>(p, qk, v, m, n_base + c, cls, img);
+            }
+          }
+        } else {
+          for (int c = half * 32; c < p.BN; c += CSTEP) {
+            const int ncols = (p.BN - c) >= 32 ? 32 : 16;
+            const uint8_t* stg = acc_tile + (q * nch + (c >> 5)) * GEMM_EPI_TILE_BYTES;
+            [[maybe_unused]] const uint8_t* rbuf = nullptr;
+            if constexpr (RES_TMA) {
+              res_issue();                              // keep GEMM_RES_NBUF - 1 loads in flight
+              mbar_wait(&rbar[rd_buf], rd_phase);       // this item's residual sub-tile (32 rows x 128 B, 128B-swizzled)
+              rbuf = rring + rd_buf * 4096;
+            }
+            const int n = n_base + c + cq * 4;
+            const bool col_ok = cq * 4 < ncols && n < p.N;
+            const unsigned cmask = __ballot_sync(0xffffffffu, col_ok);   // lanes ^8 / ^16 share cq: partners are always both in or out
+            if (col_ok) {
+              float sc[4], bi[4];
+              int4 corr4 = make_int4(0, 0, 0, 0);
+              if (MODE >= 0 || n + 3 < p.N) {
+                const float4 s4 = *reinterpret_cast<const float4*>(ep_scale + n);
+                sc[0] = s4.x; sc[1] = s4.y; sc[2] = s4.z; sc[3] = s4.w;
+                if (ep_bias) {
+                  const float4 b4 = *reinterpret_cast<const float4*>(ep_bias + n);
+                  bi[0] = b4.x; bi[1] = b4.y; bi[2] = b4.z; bi[3] = b4.w;
+                } else {
+                  bi[0] = bi[1] = bi[2] = bi[3] = 0.f;
+                }
+                if (p.corr && !conv) corr4 = *reinterpret_cast<const int4*>(p.corr + n);
+              } else {
+                int cc[4] = {0, 0, 0, 0};
+#pragma unroll
+                for (int j = 0; j < 4; ++j) {
+                  const bool ok = n + j < p.N;
+                  sc[j] = ok ? __ldg(p.scale + n + j) : 0.f;
+                  bi[j] = (ok && p.bias) ? __ldg(p.bias + n + j) : 0.f;
+                  cc[j] = (ok && p.corr && !conv) ? __ldg(p.corr + n + j) : 0;
+                }
+                corr4 = make_int4(cc[0], cc[1], cc[2], cc[3]);
+              }
+              int nq = n;   // column of the code output (per-head padded layout: attention Q/K operands)
+              if (p.oq_d > 0) { const int hq = n / p.oq_d; nq = hq * p.oq_pitch + (n - hq * p.oq_d); }
+              // Rows are finalised four at a time with everything they need from global memory (residual, conv
+              // border-class correction) fetched up front, and - on the full-tile path - without any per-row
+              // branch: the `m < M` tests split the unrolled loop into basic blocks, and with two epilogue warps
+              // per scheduler the resulting dependent-issue chains (stall_wait) bounded the small-K GEMMs.
+              const long long mrow = m_warp + rsub;
+              float* of0 = p.out ? p.out + mrow * p.ldo + n : nullptr;
+              const int oq_es = p.oq_f16 ? 2 : 1;      // bytes per emitted code
+              int8_t* oq0 = p.out_q ? p.out_q + (mrow * p.ldq + nq) * oq_es : nullptr;
+              const float* res0 = p.residual ? p.residual + mrow * p.ldr + n : nullptr;
+              const long long of_step = 4 * p.ldo, oq_step = 4 * p.ldq * oq_es, res_step = 4 * p.ldr;
+              float gsum[4] = {0.f, 0.f, 0.f, 0.f}, gsq[4] = {0.f, 0.f, 0.f, 0.f};
+              auto rows = [&](auto full_tag) {
+                constexpr bool FULL = decltype(full_tag)::value;
+#pragma unroll
+                for (int h4 = 0; h4 < 8; h4 += 4) {
+                  float4 rpre[4];
+                  int4 cpre[4];
+#pragma unroll
+                  for (int i = 0; i < 4; ++i) {
+                    const int it = h4 + i;
+                    [[maybe_unused]] const int m = m_warp + it * 4 + rsub;
+                    rpre[i] = make_float4(0.f, 0.f, 0.f, 0.f);
+                    cpre[i] = corr4;
+                    if constexpr (RES_TMA) {
+                      const int row = it * 4 + rsub;    // rows beyond M were zero-filled by the TMA unit
+                      rpre[i] = *reinterpret_cast<const float4*>(rbuf + row * 128 + ((cq ^ (row & 7)) << 4));
+                    } else if constexpr (MODE >= 0 && (MODE & EPI_RESIDUAL) != 0) {
+                      if (FULL || m < p.M) rpre[i] = *reinterpret_cast<const float4*>(res0 + it * res_step);
+                    }
+                    if constexpr (MODE >= 0 && (MODE & EPI_CORR) != 0 && (MODE & EPI_CONV) != 0)
+                      cpre[i] = __ldg(reinterpret_cast<const int4*>(p.corr + (long long)cls8[it] * p.N + n));
+                  }
+#pragma unroll
+                  for (int i = 0; i < 4; ++i) {
+                    const int it = h4 + i;
+                    const int row = it * 4 + rsub;
+                    const int m = m_warp + row;
+                    if (FULL || m < p.M) {
+                      const uint4 a4 = *reinterpret_cast<const uint4*>(stg + row * 128 + ((cq ^ (row & 7)) << 4));
+                      gemm_finalise4<MODE>(p, qk, conv, a4, sc, bi, cpre[i], rpre[i], of0 + it * of_step, oq0 + it * oq_step,
+                                           res0 + it * res_step, n, cls8[it], img8[it], gsum, gsq);
+                    }
+                  }
+                }
+              };
+              if (m_warp + 32 <= p.M) rows(std::true_type{}); else rows(std::false_type{});
+              if ((MODE < 0 || (MODE & EPI_OUT_F32) != 0) && p.gn_stats != nullptr && m_warp < p.M) {
+                // this thread holds 8 of the slab's 32 rows for 4 columns: add the other three row groups (lanes ^ 8, ^ 16),
+                // lanes 0-7 then own the slab's column sums for the chunk's 32 columns.  A row quarter wholly beyond M (the
+                // last tile of a ragged M) has no slab: gn_stats holds ceil(M / 32) of them.
+#pragma unroll
+                for (int j = 0; j < 4; ++j) {
+                  gsum[j] += __shfl_xor_sync(cmask, gsum[j], 8);
+                  gsq[j] += __shfl_xor_sync(cmask, gsq[j], 8);
+                  gsum[j] += __shfl_xor_sync(cmask, gsum[j], 16);
+                  gsq[j] += __shfl_xor_sync(cmask, gsq[j], 16);
+                }
+                if (rsub == 0) {
+                  float2* st = p.gn_stats + (long long)(m_warp >> 5) * p.ld_stats + n;
+                  if (MODE >= 0 || n + 3 < p.N) {
+                    *reinterpret_cast<float4*>(st) = make_float4(gsum[0], gsq[0], gsum[1], gsq[1]);
+                    *reinterpret_cast<float4*>(st + 2) = make_float4(gsum[2], gsq[2], gsum[3], gsq[3]);
+                  } else {
+#pragma unroll
+                    for (int j = 0; j < 4; ++j)
+                      if (n + j < p.N) st[j] = make_float2(gsum[j], gsq[j]);
+                  }
+                }
+              }
+            }
+            if constexpr (RES_TMA) {
+              fence_proxy_async();      // this buffer's generic-proxy reads are ordered before the TMA write that reuses it
+              if (++rd_buf == GEMM_RES_NBUF) { rd_buf = 0; rd_phase ^= 1; }
+            }
+            __syncwarp();
+          }
+        }
+        release();
+      }
+    };
+
+    if constexpr (!OVL) {
+      // serial schedule (gemm_overlap): the eight consumer warps run the epilogue themselves
+      // after each main loop; named barrier 1 keeps the dump behind the previous tile's last read, and the reads behind
+      // the dump
+      if constexpr (SPLITK) {
+        for (int item = blockIdx.x; item < num_tiles; item += gridDim.x) consume(item, [] {});
+      } else {
+        epilogue(
+            cw,
+            [&](const int item) {
+              consume(item, [] { named_bar_sync(1, 8 * 32); });
+              named_bar_sync(1, 8 * 32);
+            },
+            [] {});
+      }
+    } else if (warp < 12) {
+      // Overlapped schedule.  The CTA's j-th work item (j = 0, 1, ...; both sides walk the same item sequence) completes
+      // phase j of acc_full (8 consumer-warp arrivals after the dump) and then phase j of acc_empty (EPI_WARPS arrivals
+      // after the epilogue's last read).  A wait on parity P returns once the phase of parity P most recently begun has
+      // completed; a fresh barrier counts as having just completed a phase of parity 1.  So:
+      //   consumer, before dumping item j: wait(acc_empty, (j & 1) ^ 1) - j = 0 passes at once, j >= 1 waits for phase
+      //     j - 1 (the epilogue of item j - 1).  Phase j - 1 cannot be mistaken for j - 3: acc_empty cannot run more than
+      //     one phase ahead of this wait, since its phase j needs the dump of item j that follows it.
+      //   epilogue warp, before reading item j: wait(acc_full, j & 1) - phase j, the dump of item j; phase j + 1 (the
+      //     next dump) cannot complete before this warp arrives on acc_empty for item j.
+      // The arrives release and the waits acquire (CTA scope), ordering the generic-proxy tile stores before the
+      // epilogue's loads, and those loads before the next dump's stores; __syncwarp orders the other lanes' accesses
+      // before lane 0's arrive.
+      gemm_setmaxnreg<gemm_consumer_regs(MODE), gemm_launch_regs(MODE)>();
+      uint32_t j = 0;
+      for (int item = blockIdx.x; item < num_tiles; item += gridDim.x, ++j) {
+        consume(item, [&] { mbar_wait(acc_empty, (j & 1) ^ 1); });
+        __syncwarp();
+        if (lane == 0) mbar_arrive(acc_full);
+      }
+    } else {
+      gemm_setmaxnreg<gemm_epi_regs(MODE), gemm_launch_regs(MODE)>();
+      uint32_t j = 0;
+      epilogue(
+          warp - 12, [&](int) { mbar_wait(acc_full, j & 1); },
+          [&] {
+            __syncwarp();
+            if (lane == 0) mbar_arrive(acc_empty);
+            ++j;
+          });
     }
   }
 }

@@ -105,6 +105,14 @@ __device__ __forceinline__ void named_bar_sync(uint32_t id, uint32_t threads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory");
 }
 
+// ---------------------------------------------------------------- per-warpgroup register budgets
+// Executed by all 128 threads of a warpgroup: lowers (dec) or raises (inc) the warpgroup's registers per thread to R
+// (a multiple of 8 in [24, 256]).  An inc waits until enough registers have been released into the SM's pool.
+template <int R>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
+template <int R>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
+
 // ---------------------------------------------------------------- wgmma (sm_90a warpgroup MMA)
 // A warpgroup (4 consecutive warps, the first a multiple of 4) issues D[64 x N] (+)= A[64 x K] * B[N x K]^T with both
 // operands in shared memory and D in registers.  Fragment of D owned by thread t = 32 * w + l of the warpgroup:
