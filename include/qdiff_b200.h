@@ -425,6 +425,36 @@ typedef struct qd_ancestral_desc {
 int qd_ancestral_step(const qd_ancestral_desc* d, qd_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------
+ * qd_weight_scale_search -- the channel-wise 'mse' initialisation of an asymmetric n-bit weight quantizer
+ * (UniformAffineQuantizer.init_quantization_scale, qdiff/quant_layer.py:112-190), one row = one output channel.
+ *   Row r is w[r * ld + k] for k in [k0, k1) (one split-shortcut half, or the whole row).  With x_max, x_min its extremes
+ *   (no clamp to 0), candidate i = 0..79 in fp32 as the reference computes it:
+ *     s_i = (float)(1.0 - 0.01 * i)  (double, then rounded)     new_max = x_max * s_i, new_min = x_min * s_i
+ *     delta_i = (new_max - new_min) / (2^n - 1)                 zp_i = rne(-new_min / delta_i)
+ *     xq = (clamp(rne(x / delta_i) + zp_i, 0, 2^n - 1) - zp_i) * delta_i       (IEEE division, fp32)
+ *   score_i = sum over the row of |x - xq|^2.4, summed in float64 in a fixed order (the reference's 1/K factor, which
+ *   cannot change the choice, is left out).  The chosen candidate is the first one with a strictly smaller score.
+ *   Each |x - xq|^2.4 term is double pow() of the exact fp32 error: the float64 value to pow's last-bit accuracy.
+ * Outputs per row: delta[r], zero_point[r] (fp32), index[r] (0..79); score[r] (optional, NULL: not written).
+ * n_bits in [2, 8].  A row that is constant or holds a non-finite value has no candidate with a usable step (the reference
+ * leaves delta at None): the call is refused with QD_ERR_UNSUPPORTED, naming the first such row.
+ * The call synchronises `stream` to read that verdict back, so it cannot be captured into a CUDA graph.
+ * ------------------------------------------------------------------------------------------ */
+typedef struct qd_wsearch_desc {
+  const float* w;         /* [N, ld] fp32, row-major (OIHW flattened) */
+  long long ld;           /* row pitch in elements */
+  int32_t N;
+  int32_t k0, k1;         /* column range [k0, k1) of every row, 0 <= k0 < k1 <= ld */
+  int32_t n_bits;
+  float* delta;           /* [N] */
+  float* zero_point;      /* [N] */
+  int32_t* index;         /* [N] chosen candidate */
+  double* score;          /* [N] optional: the chosen candidate's score */
+} qd_wsearch_desc;
+
+int qd_weight_scale_search(const qd_wsearch_desc* d, qd_stream_t stream);
+
+/* ------------------------------------------------------------------------------------------
  * Engine: a recorded program of the ops above for one UNet (QuantModel.forward,
  * qdiff/quant_model.py:68-69 -> UNetModel.forward openaimodel.py:745-782 / Model.forward
  * ddim/models/diffusion.py:308-360).  The host graph builder (qdiff_b200/graph.py) records ops

@@ -18,13 +18,12 @@
 #include "attention_wg.cuh"
 #include "elem.cuh"
 #include "gemm_i8.cuh"
+#include "runtime.cuh"
 
-namespace {
+namespace qdr {
 
 thread_local char g_err[512] = "";
 std::atomic<long long> g_launches{0};
-constexpr int kMaxDevices = 64;
-std::atomic<int> g_num_sms[kMaxDevices];   // per device (zero-initialised): a process may drive several GPUs
 
 int fail(int code, const char* fmt, ...) {
   va_list ap;
@@ -41,25 +40,19 @@ int check_launch(const char* what) {
   return QD_OK;
 }
 
-// Every kernel launch of the library goes through here.
-// Programmatic dependent launch (cudaLaunchAttributeProgrammaticStreamSerialization on every launch + griddepcontrol.wait /
-// launch_dependents in every kernel) showed no gain inside the CUDA graphs on the previous GPU generation (not re-measured
-// on the H100), so the launches stay plain.
-template <typename... KArgs, typename... Args>
-void launch_k(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t s, Args&&... args) {
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = grid;
-  cfg.blockDim = block;
-  cfg.dynamicSmemBytes = smem;
-  cfg.stream = s;
-  cudaLaunchKernelEx(&cfg, kern, KArgs(std::forward<Args>(args))...);
-}
-
 int current_device() {
   int dev = -1;
   if (cudaGetDevice(&dev) != cudaSuccess) return -1;
   return dev;
 }
+
+}  // namespace qdr
+
+namespace {
+
+using namespace qdr;
+
+std::atomic<int> g_num_sms[kMaxDevices];   // per device (zero-initialised): a process may drive several GPUs
 
 // SM count of the CURRENT device (cached per device).
 int num_sms() {
@@ -77,20 +70,6 @@ int num_sms() {
     g_num_sms[dev].store(n, std::memory_order_relaxed);
   }
   return n;
-}
-
-// cudaFuncAttributeMaxDynamicSharedMemorySize is a PER-DEVICE attribute of a kernel: opt in once per (kernel, device).
-// `done` is the kernel instantiation's own bitmask of devices already configured.
-template <typename K>
-int ensure_smem_optin(K kern, int bytes, std::atomic<unsigned long long>& done, const char* what) {
-  const int dev = current_device();
-  if (dev < 0 || dev >= kMaxDevices) return fail(QD_ERR_CUDA, "%s: no current CUDA device", what);
-  const unsigned long long bit = 1ull << dev;
-  if (done.load(std::memory_order_acquire) & bit) return QD_OK;
-  cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
-  if (e != cudaSuccess) return fail(QD_ERR_CUDA, "%s: cudaFuncSetAttribute: %s", what, cudaGetErrorString(e));
-  done.fetch_or(bit, std::memory_order_release);
-  return QD_OK;
 }
 
 struct DeviceGuard {   // run a block on `device`, restoring the caller's current device afterwards

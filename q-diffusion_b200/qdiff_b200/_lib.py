@@ -144,10 +144,15 @@ class AncestralDesc(C.Structure):
     ]
 
 
+class WsearchDesc(C.Structure):
+    _fields_ = [("w", c_vp), ("ld", c_ll), ("N", c_i32), ("k0", c_i32), ("k1", c_i32), ("n_bits", c_i32),
+                ("delta", c_vp), ("zero_point", c_vp), ("index", c_vp), ("score", c_vp)]
+
+
 EXPORTS = [
     "qd_qgemm_i8", "qd_quantize", "qd_groupnorm_quant", "qd_groupnorm_workspace_floats", "qd_layernorm_quant",
     "qd_im2col_i8", "qd_qattention", "qd_split_bf16x3", "qd_attention_fp32", "qd_embed_tokens", "qd_lincomb3", "qd_timestep_embedding", "qd_copy2d", "qd_nchw_to_nhwc", "qd_nhwc_to_nchw", "qd_avgpool2x", "qd_upsample2x_f32", "qd_vq_lookup", "qd_softmax_rows",
-    "qd_sampler_step", "qd_ancestral_step", "qd_engine_create", "qd_engine_add_op", "qd_engine_num_ops", "qd_engine_finalize",
+    "qd_sampler_step", "qd_ancestral_step", "qd_weight_scale_search", "qd_engine_create", "qd_engine_add_op", "qd_engine_num_ops", "qd_engine_finalize",
     "qd_engine_run", "qd_engine_run_range", "qd_engine_destroy", "qd_last_error", "qd_num_sms", "qd_launch_count",
 ]
 
@@ -170,7 +175,7 @@ def lib():
     L.qd_launch_count.restype = c_ll
     for name in ("qd_qgemm_i8", "qd_quantize", "qd_groupnorm_quant", "qd_layernorm_quant", "qd_im2col_i8",
                  "qd_qattention", "qd_sampler_step", "qd_ancestral_step", "qd_split_bf16x3", "qd_attention_fp32",
-                 "qd_embed_tokens"):
+                 "qd_embed_tokens", "qd_weight_scale_search"):
         getattr(L, name).argtypes = [c_vp, c_vp]
         getattr(L, name).restype = C.c_int
     L.qd_timestep_embedding.argtypes = [c_vp, c_vp, c_i32, c_i32, c_i32, c_vp, c_vp]

@@ -24,6 +24,7 @@ class AdaRoundQuantizer(nn.Module):
         """alpha such that sigmoid-rectified(alpha) equals the fractional part (hard rounding == nearest)."""
         if self.round_mode != 'learned_hard_sigmoid':
             raise NotImplementedError(self.round_mode)
+        x = x.to(self.delta.device)        # calibration keeps delta on the CUDA device: alpha is computed there
         rest = x / self.delta - torch.floor(x / self.delta)
         self.alpha = nn.Parameter(-torch.log((self.zeta - self.gamma) / (rest - self.gamma) - 1))
 

@@ -10,8 +10,10 @@ DDIM (default), --dpm (DPM-Solver++ 2M) and -v (the 1000-step ancestral loop); t
 names the sampler and its NFE (UNet calls per image batch).  Scope (SURVEY section 8): the denoising loop on a
 calibrated checkpoint -- `--ptq --resume --cali_ckpt ckpt.pth` (the checkpoint the reference's calibration wrote; it
 carries the FP weights, the AdaRound parameters and the activation quantizers, SURVEY Appendix C, so no base checkpoint
-is needed).  Calibration itself (`--ptq` without `--resume`) and `--resume_w` are outside the hot path: those flags
-parse, and the run stops with a message naming what to do instead.
+is needed).  `--ptq --cali_iters 0` without `--resume` (and without `--quant_act`) calibrates the weight quantizers of
+the base checkpoint on the engine (qdiff_b200.calibrate), writes ckpt.pth where the reference script writes it and samples
+in the weight-only state.  Activation calibration (`--quant_act` without `--resume`), reconstruction (`--cali_iters` > 0)
+and `--resume_w` stop with a message naming what to do instead.
 
 txt2img prompts (--prompt, --from-file) are encoded by the CLIP text encoder ON THE ENGINE (qdiff_b200.text_encoder)
 when --ckpt names a file holding `cond_stage_model.transformer.*` (the SD checkpoint the reference loads): its weights
@@ -211,6 +213,8 @@ def _require_resume(args):
                          "SURVEY Appendix D Q5)")
     if args.b200_synthetic:
         return
+    if _calibrates(args):
+        return
     if args.resume_w or not args.resume:
         raise SystemExit("calibration is not part of the sampling hot path (SURVEY section 8 f4): calibrate with the "
                          "reference, then run with --resume --cali_ckpt <ckpt.pth>")
@@ -218,13 +222,47 @@ def _require_resume(args):
         raise SystemExit(f"--cali_ckpt {args.cali_ckpt!r} not found")
 
 
-def _wrap(model, args, a_sym, device):
+def _calibrates(args):
+    """--ptq without --resume / --resume_w / --quant_act: weight calibration on the engine, which is all the reference
+    computes for the weights with --cali_iters 0.  Reconstruction iterations are refused."""
+    if args.resume or args.resume_w or args.quant_act:
+        return False
+    if args.cali_iters != 0:
+        raise SystemExit(f"--cali_iters {args.cali_iters}: AdaRound reconstruction is not on the engine; --cali_iters 0 "
+                         "calibrates its starting point (the weight quantizers) on the engine")
+    return True
+
+
+def _base_state(path, what):
+    """The state dict of a base checkpoint (its `state_dict` entry when it has one); refuses a missing file."""
+    import torch
+    if not path or not os.path.isfile(path):
+        raise SystemExit(f"{what}: base checkpoint {path!r} not found (nothing is downloaded)")
+    sd = torch.load(path, map_location="cpu", weights_only=False)
+    return sd.get("state_dict", sd) if isinstance(sd, dict) else sd
+
+
+def _wrap(model, args, a_sym, device, scale_method='max', out_dir="."):
+    """QuantModel over `model`.  --resume: quantizer parameters from --cali_ckpt.  Otherwise (_calibrates: `model` holds
+    the base weights) the weight quantizers are initialised on the engine with the reference script's scale_method, and
+    the reference-format checkpoint is written as <out_dir>/ckpt.pth, where the reference script writes it."""
     import qdiff_b200 as qd
-    wq = {'n_bits': args.weight_bit, 'channel_wise': True, 'scale_method': 'max'}
+    from . import calibrate
+    calib = not args.resume
+    wq = {'n_bits': args.weight_bit, 'channel_wise': True, 'scale_method': scale_method if calib else 'max'}
     aq = {'n_bits': args.act_bit, 'symmetric': a_sym, 'channel_wise': False, 'scale_method': 'max',
           'leaf_param': args.quant_act}
     qnn = qd.QuantModel(model=model, weight_quant_params=wq, act_quant_params=aq, sm_abit=args.sm_abit)
-    qd.resume_cali_model(qnn, args.cali_ckpt, None, args.quant_act, "qdiff", cond=bool(getattr(args, "cond", False)))
+    if calib:
+        print(f"--cali_data_path {getattr(args, 'cali_data_path', None)!r} is not read: weight initialisation (--cali_iters 0) "
+              "does not depend on calibration data")
+        calibrate.init_weight_quantizers(qnn, device)
+        os.makedirs(out_dir, exist_ok=True)
+        path = os.path.join(out_dir, "ckpt.pth")
+        calibrate.save_cali_ckpt(qnn, path)
+        print(f"calibrated weight quantizers ({scale_method}, W{args.weight_bit}) -> {path}")
+    else:
+        qd.resume_cali_model(qnn, args.cali_ckpt, None, args.quant_act, "qdiff", cond=bool(getattr(args, "cond", False)))
     if args.verbose:
         print(qnn)
     return qnn
@@ -350,7 +388,20 @@ def run_ddim(args):
                                             in_channels=m["in_channels"], image_size=size,
                                             resamp_with_conv=m.get("resamp_with_conv", True), split_shortcut=args.split,
                                             num_diffusion_timesteps=d["num_diffusion_timesteps"]))
-        qnn = _wrap(model, args, args.a_sym, dev)
+        if _calibrates(args):
+            # sample_diffusion_ddim.py:113-121: ddim/functions/ckpt_util.get_ckpt_path("ema_<dataset>"), never downloaded
+            data = cfg["data"]
+            name = "cifar10" if data.get("dataset") == "CIFAR10" else f"lsun_{data.get('category')}".replace(
+                "church_outdoor", "church")
+            sub = {"cifar10": "ema_diffusion_cifar10_model/model-790000.ckpt",
+                   "lsun_bedroom": "ema_diffusion_lsun_bedroom_model/model-2388000.ckpt",
+                   "lsun_cat": "ema_diffusion_lsun_cat_model/model-1761000.ckpt",
+                   "lsun_church": "ema_diffusion_lsun_church_model/model-4432000.ckpt"}.get(name)
+            if sub is None:
+                raise SystemExit(f"no pretrained DDIM checkpoint is defined for dataset {name!r}")
+            cache = os.environ.get("XDG_CACHE_HOME", os.path.expanduser("~/.cache"))
+            model.load_state_dict(_base_state(os.path.join(cache, "diffusion_models_converted", sub), "DDIM"), strict=True)
+        qnn = _wrap(model, args, args.a_sym, dev, 'max', args.logdir if args.logdir != "none" else ".")
         batch = cfg["sampling"]["batch_size"]
     if d.get("beta_schedule", "linear") != "linear":
         raise SystemExit("only the linear beta schedule of the reference's configs is supported")
@@ -428,7 +479,16 @@ def run_ldm(args):
         cfg = _ldm_config(args)["model"]["params"]
         up = dict(cfg["unet_config"]["params"])
         model = unet.UNetModel(**up)
-        qnn = _wrap(model, args, args.a_sym, dev)
+        if _calibrates(args):
+            # sample_diffusion_ldm.py:384-450: -r names the checkpoint (or its logdir's model.ckpt); EMA weights
+            base = args.resume_base
+            sd = _base_state(base if os.path.isfile(base) else os.path.join(base.rstrip("/"), "model.ckpt"), "-r")
+            ema = {k: sd["model_ema." + ("diffusion_model." + k).replace(".", "")] for k in model.state_dict()
+                   if "model_ema." + ("diffusion_model." + k).replace(".", "") in sd}
+            if len(ema) != len(model.state_dict()):
+                raise SystemExit(f"-r {base!r}: the checkpoint has no EMA copy (model_ema.*) of every UNet parameter")
+            model.load_state_dict(ema, strict=True)
+        qnn = _wrap(model, args, args.a_sym, dev, 'mse', args.logdir if args.logdir != "none" else ".")
         ch, size = cfg["channels"], cfg["image_size"]
         sched = dict(timesteps=cfg.get("timesteps", 1000), linear_start=cfg.get("linear_start", 1e-4),
                      linear_end=cfg.get("linear_end", 2e-2))
@@ -548,7 +608,12 @@ def run_txt2img(args):
         cfg = _load_yaml(args.config)["model"]["params"]
         model = unet.UNetModel(**dict(cfg["unet_config"]["params"]))
         model.split = bool(args.split)
-        qnn = _wrap(model, args, False, dev)
+        if _calibrates(args):
+            # txt2img.py:57-66, 358: the UNet of --ckpt, keys model.diffusion_model.*
+            sd = _base_state(args.ckpt, "--ckpt")
+            pre = "model.diffusion_model."
+            model.load_state_dict({k[len(pre):]: v for k, v in sd.items() if k.startswith(pre)}, strict=True)
+        qnn = _wrap(model, args, False, dev, 'mse', args.outdir)
         sched = dict(timesteps=cfg.get("timesteps", 1000), linear_start=cfg["linear_start"], linear_end=cfg["linear_end"])
         ctx_shape = (77, cfg["unet_config"]["params"]["context_dim"])
     Sampler = samplers.PLMSSampler if args.plms else samplers.DDIMSampler

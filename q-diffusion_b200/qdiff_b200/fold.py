@@ -25,18 +25,22 @@ def weight_codes(w, delta, zero_point, n_bits, alpha=None):
     return torch.clamp(x_int + zp, 0, 2 ** n_bits - 1)
 
 
-def init_weight_qparams_max(w, n_bits):
+def init_weight_qparams_max(w, n_bits, scale_method='max'):
     """'max' init of the channel-wise weight quantizer (qdiff/quant_layer.py:112-160), vectorised.
 
-    Per output channel: delta = (max - min) / (2^n - 1), zp = rne(-min(min,0) / delta).
+    Per output channel: delta = (max - min) / (2^n - 1), zp = rne(-min(min,0) / delta).  A scale_method containing
+    'scale' first multiplies min(min,0) by (n + 2) / 8, which moves only the zero point (quant_layer.py:145-147).
     """
     w2 = w.detach().to(torch.float32).reshape(w.shape[0], -1)
     w_max = w2.max(dim=1).values
     w_min = w2.min(dim=1).values
     # the reference does this arithmetic on python floats (double) and casts delta to fp32 last
-    delta64 = (w_max.double() - w_min.double()) / (2 ** n_bits - 1)
+    # divided by a tensor: torch's CUDA kernels divide by a Python scalar as a multiply by its reciprocal
+    delta64 = (w_max.double() - w_min.double()) / torch.tensor(2.0 ** n_bits - 1, dtype=torch.float64, device=w.device)
     delta64 = torch.where(delta64 < 1e-8, torch.full_like(delta64, 1e-8), delta64)
     x_min = torch.minimum(w_min, torch.zeros_like(w_min)).double()
+    if 'scale' in scale_method:
+        x_min = x_min * (n_bits + 2) / 8
     # python round() on a float is round-half-even, same as torch.round
     zp = torch.round(-x_min / delta64).to(torch.float32)
     return delta64.to(torch.float32), zp

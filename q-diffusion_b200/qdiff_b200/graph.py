@@ -441,6 +441,11 @@ class Builder:
         if ent is not None and (not self.want_specs or ent.get("w8") or "ws_cpu" in ent):
             return ent
         ws, delta_w = self._fold(qm, cols, suffix)
+        if part is None and (float(ws.min()) < -256 or float(ws.max()) > 255):
+            # a zero point outside [0, 2^n - 1] (single-signed channels): floor(ws / 2) would not fit the s8 operand
+            raise RuntimeError(f"{label}: weight codes minus zero point span [{float(ws.min()):.0f}, "
+                               f"{float(ws.max()):.0f}]; the INT8 GEMM takes [-256, 255] exactly (zero point outside "
+                               "the code range): this layer cannot run exactly in the INT8 state")
         kdup = 1
         if part is None and float(ws.abs().max()) > 127:
             # 8-bit weights: wq - zw spans [-255, 255].  One GEMM whose reduction runs twice over the activation, against
@@ -1236,6 +1241,11 @@ class WeightOnlyBuilder(Builder):
             if passes is _CODES:
                 w, delta_w = self._fold(qm, cols, suffix)
                 planes = (w.to(torch.bfloat16),)
+                if not torch.equal(planes[0].float(), w):
+                    # a zero point outside [0, 2^n - 1] (single-signed channels) can push |wq - zp| past 256
+                    raise RuntimeError(f"{label}: weight codes minus zero point span [{float(w.min()):.0f}, "
+                                       f"{float(w.max()):.0f}], not exact in bfloat16 (zero point outside the code "
+                                       "range): this layer cannot run exactly in the weight-only state")
             else:
                 w = qm.weight.detach().to(self.dev, torch.float32)
                 w = w if cols is None else w[:, cols[0]:cols[1], ...]

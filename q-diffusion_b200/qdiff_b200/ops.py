@@ -9,7 +9,7 @@ import torch
 
 from . import _lib
 from ._lib import (AttentionDesc, AttentionFpDesc, EmbedDesc, GemmDesc, GroupNormDesc, Im2colDesc, LayerNormDesc, MiscDesc, QParams,
-                   QuantizeDesc, SamplerDesc, SplitDesc, check, lib, ptr, stream_ptr)
+                   QuantizeDesc, SamplerDesc, SplitDesc, WsearchDesc, check, lib, ptr, stream_ptr)
 
 
 def qparams(delta, zero_point, qmin, qmax):
@@ -251,3 +251,24 @@ def timestep_embedding(t, dim, mode):
     check(lib().qd_timestep_embedding(ptr(t), ptr(freqs), t.shape[0], dim, mode, ptr(out), stream_ptr()),
           "qd_timestep_embedding")
     return out
+
+
+def weight_scale_search(w, n_bits, cols=None, with_score=False):
+    """Channel-wise 'mse' weight scale search (qd_weight_scale_search) on the rows of a CUDA weight tensor [N, ...] (each
+    output channel's weights contiguous, as PyTorch stores them), over the flattened columns `cols` = (k0, k1) or all.
+    Returns (delta [N] fp32, zero_point [N] fp32, index [N] int32, score [N] float64 or None).  Synchronises the stream;
+    raises RuntimeError (status QD_ERR_UNSUPPORTED) when a row is constant or not finite."""
+    _require_cuda(w)
+    w2 = w.detach().to(torch.float32).reshape(w.shape[0], -1).contiguous()
+    N, K = w2.shape
+    k0, k1 = (0, K) if cols is None else (int(cols[0]), int(cols[1]))
+    delta = torch.empty(N, device=w.device, dtype=torch.float32)
+    zp = torch.empty_like(delta)
+    index = torch.empty(N, device=w.device, dtype=torch.int32)
+    score = torch.empty(N, device=w.device, dtype=torch.float64) if with_score else None
+    d = WsearchDesc()
+    d.w, d.ld, d.N, d.k0, d.k1, d.n_bits = ptr(w2), K, N, k0, k1, int(n_bits)
+    d.delta, d.zero_point, d.index, d.score = ptr(delta), ptr(zp), ptr(index), ptr(score)
+    with torch.cuda.device(w.device):
+        check(lib().qd_weight_scale_search(C.byref(d), stream_ptr()), "qd_weight_scale_search")
+    return delta, zp, index, score

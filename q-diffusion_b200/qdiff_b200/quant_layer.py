@@ -71,13 +71,22 @@ class UniformAffineQuantizer(nn.Module):
     def init_quantization_scale(self, x, channel_wise=False):
         """'max' / 'mse' scale search (reference quant_layer.py:112-181)."""
         if channel_wise:
+            shape = (-1,) + (1,) * (x.dim() - 1)
+            if x.is_cuda and not self.sym and not self.always_zero and ('max' in self.scale_method or
+                                                                        self.scale_method == 'mse'):
+                # every channel at once on the device: the vectorised 'max' rule, or the 'mse' search kernel
+                from . import fold, ops
+                if 'max' in self.scale_method:
+                    d, z = fold.init_weight_qparams_max(x, self.n_bits, self.scale_method)
+                else:
+                    d, z, _, _ = ops.weight_scale_search(x, self.n_bits)
+                return d.reshape(shape), z.reshape(shape)
             xc = x.detach()
             deltas, zps = [], []
             for c in range(xc.shape[0]):
                 d, z = self.init_quantization_scale(xc[c], False)
                 deltas.append(torch.as_tensor(d, dtype=x.dtype, device=x.device))
                 zps.append(torch.as_tensor(float(z), dtype=x.dtype, device=x.device))
-            shape = (-1,) + (1,) * (x.dim() - 1)
             return torch.stack(deltas).reshape(shape), torch.stack(zps).reshape(shape)
         if self.leaf_param:
             self.x_min, self.x_max = x.data.min(), x.data.max()

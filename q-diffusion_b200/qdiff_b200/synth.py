@@ -47,38 +47,13 @@ def calib_inputs(name, batch=1, seed=1234):
     return x, t, ctx
 
 
-def _split_points(model, spec):
-    """{module name: split} for the skip 1x1 convs that see a concatenated input (reference
-    openaimodel.py:771-777 / ddim diffusion.py:338-346): split = channels of h before the concat."""
-    out = {}
-    if not spec["split"]:
-        return out
-    if spec["family"] == "ddim":
-        ch, mult, nrb = model.ch, tuple(model.config.model.ch_mult), model.num_res_blocks
-        block_in = ch * mult[-1]
-        for lv in reversed(range(len(mult))):
-            for ib in range(nrb + 1):
-                blk = model.up[lv].block[ib]
-                if blk.in_channels != blk.out_channels and lv < 4:
-                    out[f"up.{lv}.block.{ib}.nin_shortcut"] = block_in
-                block_in = ch * mult[lv]
-        return out
-    h_ch = model.middle_block[0].out_channels
-    for i, blk in enumerate(model.output_blocks):
-        res = blk[0]
-        if not isinstance(res.skip_connection, torch.nn.Identity):
-            out[f"output_blocks.{i}.0.skip_connection"] = h_ch
-        h_ch = res.out_channels
-    return out
-
-
 def weight_ckpt(name, model, prefix="model."):
     """ckpt.pth-format dict (SURVEY Appendix C) with weights, channel-wise 'max' weight quantizers and
     seeded AdaRound alpha (+-1, stored int8).  Activation entries are added by the caller."""
     spec = SPECS[name]
     g = torch.Generator().manual_seed(spec["seed"] + 7)
     sd = model.state_dict()
-    splits = _split_points(model, spec)
+    splits = unet.split_points(model)
     ckpt = {prefix + k: v for k, v in sd.items()}
     for k, w in sd.items():
         if not k.endswith(".weight") or w.dim() < 2:

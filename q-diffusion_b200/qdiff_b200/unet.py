@@ -348,6 +348,35 @@ def build_unet(name_or_family, **overrides):
     return UNetModel(**params)
 
 
+def split_points(model):
+    """{module name: split} for the skip 1x1 convs that see a concatenated input when the model quantises split
+    shortcuts (reference openaimodel.py:771-777 / ddim diffusion.py:338-346): split = channels of h before the concat.
+    The flag is the model's own: config.split_shortcut (DDIM Model) or .split (UNetModel).  Works on the bare module tree
+    and on one wrapped by QuantModel (the block wrappers keep the channel attributes)."""
+    out = {}
+    if hasattr(model, "output_blocks"):
+        if not getattr(model, "split", False):
+            return out
+        h_ch = model.middle_block[0].out_channels
+        for i, blk in enumerate(model.output_blocks):
+            res = blk[0]
+            if not isinstance(res.skip_connection, nn.Identity):
+                out[f"output_blocks.{i}.0.skip_connection"] = h_ch
+            h_ch = res.out_channels
+        return out
+    if not getattr(model.config, "split_shortcut", False):
+        return out
+    ch, mult, nrb = model.ch, tuple(model.config.model.ch_mult), model.num_res_blocks
+    block_in = ch * mult[-1]
+    for lv in reversed(range(len(mult))):
+        for ib in range(nrb + 1):
+            blk = model.up[lv].block[ib]
+            if blk.in_channels != blk.out_channels and lv < 4:
+                out[f"up.{lv}.block.{ib}.nin_shortcut"] = block_in
+            block_in = ch * mult[lv]
+    return out
+
+
 def randomize_(model, seed=0, std_zero_init=0.02):
     """Seeded synthetic weights (there are no pretrained checkpoints offline): default torch inits
     under manual_seed, with every all-zero weight tensor (the reference's zero_module convs,
