@@ -100,6 +100,7 @@ class _FirstStage(_NoForward):
     """Shared engine plumbing: program cache, decode()."""
     act_quant_params = {}
     weight_quant_params = {"n_bits": 32}
+    record_op_specs = False      # tests: describe every op of a lowered program for the in-situ per-op check
 
     def _init_engine_state(self, precision, cuda_graph):
         if precision not in graph._PASSES:
@@ -228,9 +229,10 @@ class FirstStageBuilder(graph.WeightOnlyBuilder):
             self.keep.append(t)
             for sl in range(nact):
                 self.misc(_lib.QD_OP_COPY2D, planes.ptr + 2 * wp * Cp, t.data_ptr() + 2 * sl * Cp, rows, Cp // 2,
-                          ld_src=3 * Cp // 2, ld_dst=nact * Cp // 2, label=f"{label}.tile{wp}.{sl}")
+                          ld_src=3 * Cp // 2, ld_dst=nact * Cp // 2, label=f"{label}.tile{wp}.{sl}",
+                          spec=dict(kind="plane_tile", src=planes, plane=wp, dst=t, slot=sl, Cp=Cp) if self.want_specs else None)
             tiles.append((t, nact))
-        return dict(tiles=tiles, scale=scale, bias=None, N=rows, N_real=rows, taps=1)
+        return dict(tiles=tiles, scale=scale, bias=None, N=rows, N_real=rows, taps=1, passes=passes, planes=planes)
 
     def attn_products_tc(self, q, k, v, T, C_, label):
         """softmax(q k^T C^-1/2) v with both products as bfloat16-plane GEMMs on wgmma (fp32 accumulation), per image:
@@ -251,10 +253,13 @@ class FirstStageBuilder(graph.WeightOnlyBuilder):
             pk = self.split3(kb, lb + ".k.split")
             S = self.new_f32(T, T)
             self.plane_gemm(self._plane_tiles(pk, T, aq.Cp, graph._PASSES[6], sc_qk, lb + ".k"), aq, lb + ".qk", out=S)
-            self.misc(_lib.QD_OP_SOFTMAX_ROWS, S.ptr, S.ptr, T, T, ld_src=S.ld, ld_dst=S.ld, label=lb + ".softmax")
+            self.misc(_lib.QD_OP_SOFTMAX_ROWS, S.ptr, S.ptr, T, T, ld_src=S.ld, ld_dst=S.ld, label=lb + ".softmax",
+                      spec=dict(kind="softmax_rows", x=S) if self.want_specs else None)
             ap = self.split3(S, lb + ".p.split")
             vt = self.new_f32(C_, T)
-            self.misc(_lib.QD_OP_NHWC_TO_NCHW, self.contig(vb, lb + ".v").ptr, vt.ptr, 1, C_, T, label=lb + ".v.t")
+            vc = self.contig(vb, lb + ".v")
+            self.misc(_lib.QD_OP_NHWC_TO_NCHW, vc.ptr, vt.ptr, 1, C_, T, label=lb + ".v.t",
+                      spec=dict(kind="nhwc_to_nchw", src=vc, dst=vt.t.view(1, C_, T)) if self.want_specs else None)
             pv = self.split3(vt, lb + ".vt.split")
             ob = graph.Act(o_all.t[rows], T, C_, ld=o_all.ld)
             self.plane_gemm(self._plane_tiles(pv, C_, ap.Cp, graph._PASSES[self.precision], ones_c, lb + ".vt"), ap, lb + ".pv",
@@ -268,14 +273,15 @@ class FirstStageBuilder(graph.WeightOnlyBuilder):
         t_in = torch.zeros(B, dtype=torch.float32, device=self.dev)
         self.keep += [x_in, t_in]
         zh = self.new_f32(B * H * W, zc)
-        self.misc(_lib.QD_OP_NCHW_TO_NHWC, x_in.data_ptr(), zh.ptr, B, zc, H * W, label="z.nhwc")
+        self.misc(_lib.QD_OP_NCHW_TO_NHWC, x_in.data_ptr(), zh.ptr, B, zc, H * W, label="z.nhwc",
+                  spec=dict(kind="nchw_to_nhwc", src=x_in, dst=zh) if self.want_specs else None)
         if quantize:
             cb = fs.quantize.embedding.weight.detach().to(self.dev, torch.float32).contiguous()
             if cb.shape[1] != zc:
                 raise ValueError(f"codebook dim {cb.shape[1]} != latent channels {zc}")
             zq = self.new_f32(B * H * W, zc)
             self.misc(_lib.QD_OP_VQ_LOOKUP, zh.ptr, zq.ptr, B * H * W, zc, cb.shape[0], ld_src=zh.ld, ld_dst=zq.ld,
-                      label="quantize", aux=cb)
+                      label="quantize", aux=cb, spec=dict(kind="vq_lookup", src=zh, dst=zq, cb=cb) if self.want_specs else None)
             zh = zq
         hw = (H, W)
         h = self.conv(fs.post_quant_conv, zh, "post_quant_conv", hw)
@@ -299,15 +305,17 @@ class FirstStageBuilder(graph.WeightOnlyBuilder):
                     h = self.plane_gemm(up.conv, a, self.key(up.conv), hw=hw)
                 else:
                     big = self.new_f32(4 * h.rows, h.cols)
-                    self.misc(_lib.QD_OP_UPSAMPLE2X, self.contig(h, "up").ptr, big.ptr, B, hw[0], hw[1], h.cols,
-                              label=self.key(up) + ".nearest")
+                    hc = self.contig(h, "up")
+                    self.misc(_lib.QD_OP_UPSAMPLE2X, hc.ptr, big.ptr, B, hw[0], hw[1], h.cols, label=self.key(up) + ".nearest",
+                              spec=dict(kind="upsample2x", src=hc, dst=big, B=B, H=hw[0], W=hw[1]) if self.want_specs else None)
                     h, hw = big, (2 * hw[0], 2 * hw[1])
             self.traces[f"up.{lv}"] = (h, hw)
         hn = self.gn_f32(h, dec.norm_out, hw[0] * hw[1], True, "decoder.norm_out")
         o = self.conv(dec.conv_out, hn, "decoder.conv_out", hw)
         out = torch.zeros((B, o.cols, hw[0], hw[1]), dtype=torch.float32, device=self.dev)     # o.cols: out_ch padded to 4
         self.keep.append(out)
-        self.misc(_lib.QD_OP_NHWC_TO_NCHW, o.ptr, out.data_ptr(), B, o.cols, hw[0] * hw[1], label="image.nchw")
+        self.misc(_lib.QD_OP_NHWC_TO_NCHW, o.ptr, out.data_ptr(), B, o.cols, hw[0] * hw[1], label="image.nchw",
+                  spec=dict(kind="nhwc_to_nchw", src=o, dst=out) if self.want_specs else None)
         return x_in, t_in, out[:, :int(dec.conv_out.weight.shape[0])]
 
 

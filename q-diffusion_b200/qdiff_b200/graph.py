@@ -1275,6 +1275,14 @@ class WeightOnlyBuilder(Builder):
                 torch.nn.functional.pad(b.detach().to(self.dev, torch.float32), (0, ent["N"] - ent["N_real"]))
         return ent
 
+    def _module_keys(self, op):
+        """Keys of the modules whose weight a plane GEMM multiplies (a row view: its module; fused q/k/v: all three)."""
+        if id(op) in self.names:
+            return (self.key(op),)
+        if hasattr(op, "qm"):
+            return (self.key(op.qm),)
+        return tuple(self.key(m) for m in op.parts)
+
     def plane_gemm(self, op, a, label, *, hw=None, im2col=None, rows_per_batch=None, rowvec=None, residual=None,
                    out=None, accumulate_into=None, use_bias=True, cols=None, suffix=""):
         """Record y = x W^T [+ bias] [+ rowvec] [+ residual] on the bfloat16 planes `a` of x (split3): one accumulating
@@ -1310,7 +1318,7 @@ class WeightOnlyBuilder(Builder):
                                  pad_top=pad_tl[0], pad_left=pad_tl[1], pad_code=0, ld_dst=9 * cbytes)
             self.add(_lib.QD_OP_IM2COL, di, label + ".im2col",
                      spec=dict(kind="im2col_bytes", src=a, dst=src, B=self.B, H=H, W=Wd, Ho=Ho, Wo=Wo, stride=stride,
-                               pad_tl=pad_tl, cbytes=cbytes) if codes else None)
+                               pad_tl=pad_tl, cbytes=cbytes) if codes or self.want_specs else None)
         elif hw is not None and taps == 9:
             conv_bhw = (self.B, hw[0], hw[1])
         if rows_per_batch is None:
@@ -1324,6 +1332,19 @@ class WeightOnlyBuilder(Builder):
                         C=a.C, taps=taps, im2col=im2col is not None, conv_bhw=conv_bhw, ws=W["ws_cpu"],
                         scale=scale.detach().cpu(), bias=None if bias is None else bias.detach().cpu(), rowvec=rowvec,
                         residual=res, rows_per_batch=rows_per_batch, out=o, N=N)
+        elif self.want_specs:
+            # one logical op over all launches of the pass table: the first launch carries the spec, the others a marker
+            if isinstance(op, dict):
+                w_cpu, w_planes, keys = None, op["planes"], ()
+            else:
+                w_cpu = op.weight.detach().to("cpu", torch.float32)
+                w_cpu = w_cpu if cols is None else w_cpu[:, cols[0]:cols[1]]
+                w_planes, keys = None, self._module_keys(op)
+            spec = dict(kind="gemm_fp", launches=len(W["tiles"]), keys=keys, a=src, Cp=a.Cp, C=a.C, taps=taps,
+                        im2col=im2col is not None, conv_bhw=conv_bhw, passes=passes if not isinstance(op, dict) else op["passes"],
+                        tiles=W["tiles"], w=w_cpu, w_planes=w_planes, scale=scale.detach().cpu(),
+                        bias=None if bias is None else bias.detach().cpu(), rowvec=rowvec, residual=res,
+                        rows_per_batch=rows_per_batch, out=o, N=N, N_real=W["N_real"])
         for i, (tile, slots) in enumerate(W["tiles"]):
             if i:
                 rowvec, res = None, o
@@ -1341,7 +1362,8 @@ class WeightOnlyBuilder(Builder):
                 d.residual = res.ptr
             d.out = o.ptr
             self.add(_lib.QD_OP_GEMM, d, label + (f".pass{i}" if i else ""),
-                     flops=0 if i else 2 * M * W["N_real"] * a.C * taps, spec=None if i else spec)
+                     flops=0 if i else 2 * M * W["N_real"] * a.C * taps,
+                     spec=spec if not i else (dict(kind="gemm_fp_pass") if spec is not None else None))
         self.layer_traces[label] = o
         return o
 

@@ -299,6 +299,7 @@ class _Fused:
     """q/k/v projections as one linear: weights and biases concatenated along the output rows."""
 
     def __init__(self, lins):
+        self.parts = tuple(lins)
         self.weight = torch.cat([m.weight.detach() for m in lins])
         self.bias = torch.cat([m.bias.detach() for m in lins])
 
@@ -309,6 +310,7 @@ class FrozenCLIPEmbedder(nn.Module):
     by tensor identity and version, DESIGN section 2: a reused buffer would leave it on stale K/V)."""
     act_quant_params = {}
     weight_quant_params = {"n_bits": 32}
+    record_op_specs = False      # tests: describe every op of a lowered program for the in-situ per-op check
 
     def __init__(self, vocab_size=49408, width=768, layers=12, mlp=3072, max_positions=77, heads=None,
                  max_length=MAX_LENGTH, layer_norm_eps=1e-5, tokenizer=None, cuda_graph=True, max_programs=4):
@@ -412,7 +414,8 @@ class TextEncoderBuilder(graph.WeightOnlyBuilder):
         tok, pos = self.wcache[key]
         self.keep += [ids_in, tok, pos]
         h = self.new_f32(B * T, C_)
-        self.add(_lib.QD_OP_EMBED, ops.embed_desc(ids_in, tok, pos, h.t, B=B, T=T, ld_out=h.ld), "embeddings")
+        self.add(_lib.QD_OP_EMBED, ops.embed_desc(ids_in, tok, pos, h.t, B=B, T=T, ld_out=h.ld), "embeddings",
+                 spec=dict(kind="embed", ids=ids_in, tok=tok, pos=pos, out=h, B=B, T=T) if self.want_specs else None)
         for i, layer in enumerate(tm.encoder.layers):
             k = f"encoder.layers.{i}"
             at = layer.self_attn
@@ -438,6 +441,9 @@ class TextProgram:
 
     def _launch(self):
         check(lib().qd_engine_run(self.engine, _lib.stream_ptr()), "qd_engine_run")
+
+    def run_range(self, first, last):
+        check(lib().qd_engine_run_range(self.engine, first, last, _lib.stream_ptr()), "qd_engine_run_range")
 
     def run(self, ids):
         self.ids_in.copy_(ids.reshape(-1).to(self.ids_in.device, torch.int32))

@@ -41,6 +41,7 @@ import math
 import os
 import re
 import tempfile
+import time
 import zlib
 
 import pytest
@@ -272,14 +273,19 @@ def _norm(name):
 
 def _launch(fn, restore=()):
     """fn() under torch.profiler; returns the normalised names of the qd:: kernels that ran.  The profiler occasionally
-    records no kernel for a call this short: the buffers in `restore` (in-place outputs) are then reset and the call
-    repeated, at most 6 times."""
+    records no kernel for a call this short (late in a long process it drops kernels whose converted timestamps fall
+    outside its window: the call runs test_gemm_matrix_gpu.PROFILE_MARGIN(attempt) seconds inside it on either side): the buffers in
+    `restore` (in-place outputs) are then reset and the call repeated with a wider margin, at most 6 times."""
     from torch.profiler import ProfilerActivity, profile
+    from tests.test_gemm_matrix_gpu import PROFILE_MARGIN
     saved = [t.clone() for t in restore]
-    for _ in range(6):
+    for attempt in range(6):
         with profile(activities=[ProfilerActivity.CPU, ProfilerActivity.CUDA]) as prof:
+            torch.cuda.synchronize()
+            time.sleep(PROFILE_MARGIN(attempt))
             fn()
             torch.cuda.synchronize()
+            time.sleep(PROFILE_MARGIN(attempt))
         names = {n for n in (_norm(e.name) for e in prof.events() if "qd::" in e.name and "_kernel" in e.name) if n}
         if names:
             break

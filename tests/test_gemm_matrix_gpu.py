@@ -33,6 +33,7 @@ import math
 import os
 import re
 import tempfile
+import time
 import zlib
 
 import pytest
@@ -256,6 +257,11 @@ INSTANTIATIONS = {
 # ---------------------------------------------------------------------------------------------------- running a case
 SEEN = set()       # (MODE, W4) pairs the profiler saw in this session
 RETRIES = [0]      # calls repeated because the profiler recorded no kernel
+
+
+def PROFILE_MARGIN(attempt):
+    """Seconds of host time kept inside the profiler window before the launch and after the synchronise."""
+    return 0.01 * 4 ** attempt
 _KERNEL = re.compile(r"gemm_i8_kernel<\s*(?:\(int\))?\s*(-?\d+)\s*,\s*(?:\(bool\))?\s*(true|false|1|0)\s*>")
 
 
@@ -266,16 +272,21 @@ def _sms():
 
 def _launch(desc, outs):
     """One qd_qgemm_i8 call under torch.profiler; returns the (MODE, W4) pairs and whether splitk_finish_kernel ran.  The
-    profiler occasionally records no kernel for a call this short; the output buffers (which may also be the residual)
-    are then restored and the call repeated, at most 6 times."""
+    profiler drops device activity whose converted timestamp falls outside its capture window, and late in a long process
+    the GPU-to-host clock conversion drifts far enough for that to hit a lone kernel; the call runs PROFILE_MARGIN(attempt)
+    seconds inside the window on either side.  When the profiler still recorded no kernel, the output buffers (which may
+    also be the residual) are restored and the call repeated with a wider margin, at most 6 times."""
     from torch.profiler import ProfilerActivity, profile
     from qdiff_b200 import ops
     saved = [t.clone() for t in outs]
-    for _ in range(6):
+    for attempt in range(6):
         with profile(activities=[ProfilerActivity.CPU, ProfilerActivity.CUDA]) as prof:
+            torch.cuda.synchronize()
+            time.sleep(PROFILE_MARGIN(attempt))
             ops.qgemm(desc)
             torch.cuda.synchronize()
             [t.cpu() for t in outs]
+            time.sleep(PROFILE_MARGIN(attempt))
         names = {e.name for e in prof.events() if "gemm_i8_kernel" in e.name or "splitk_finish_kernel" in e.name}
         if names:
             break
