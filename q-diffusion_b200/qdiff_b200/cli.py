@@ -34,6 +34,12 @@ Extra flags of this implementation (all prefixed so they cannot collide with fut
                               FILE (a first-stage or full LDM / SD checkpoint: keys `decoder.*`, `post_quant_conv.*`,
                               `quantize.embedding.weight`, optionally prefixed `first_stage_model.`), or seeded synthetic
                               weights with --b200_synthetic.  --b200_decode_precision 1|3|6: bfloat16 plane products per MAC.
+    --b200_cali_data_out FILE sample the FULL-PRECISION UNet (set_quant_state(False, False)) of the base checkpoint the
+                              --cali_iters 0 path loads (or of --b200_synthetic) and write the timestep-aware calibration
+                              set of the run to FILE, in the format the reference's --cali_data_path reads
+                              (qdiff_b200.cali_data).  The samples are saved as usual.  Not with --ptq, nor with a sampler
+                              whose steps are not recorded (--dpm, -v, --sample_type ddpm_noisy | dpm_solver).  The scripts
+                              parse it through script_parser; the sampling parsers themselves do not carry it.
 Multi-GPU: run under `python -m torch.distributed.run`; the batch is sharded by images, every rank draws the full-batch
 noise from the seed and keeps its slice, rank 0 gathers and saves (qdiff_b200/dist.py).
 """
@@ -74,6 +80,9 @@ _B200 = [
     (("--b200_first_stage",), dict(type=str, default=None, help="first-stage checkpoint for --b200_decode")),
     (("--b200_decode_precision",), dict(type=int, default=3, choices=[1, 3, 6], help="bfloat16 plane products per MAC of the decoder")),
 ]
+# the calibration-data run is a mode of the scripts, not a sampling option: script_parser adds it to a sampling parser
+_CALI_DATA_OUT = (("--b200_cali_data_out",), dict(type=str, default=None,
+                                                   help="sample the full-precision UNet and write its per-step inputs (calibration data) here"))
 
 
 def _add(parser, table):
@@ -169,6 +178,18 @@ def txt2img_parser():
     return p
 
 
+def script_parser(parser):
+    """What the scripts parse: a sampling parser (ddim_parser, ldm_parser, txt2img_parser) plus --b200_cali_data_out.
+    The run_* functions accept either namespace; one without the flag is a sampling run."""
+    _add(parser, [_CALI_DATA_OUT])
+    return parser
+
+
+def _cali_out(args):
+    """--b200_cali_data_out of a script_parser namespace; None for a plain sampling namespace."""
+    return getattr(args, "b200_cali_data_out", None)
+
+
 def surface(parser):
     """{dest: {flags, default, type, nargs, choices, required, action}} -- compared with the reference by tests."""
     out = {}
@@ -222,6 +243,18 @@ def _require_resume(args):
         raise SystemExit(f"--cali_ckpt {args.cali_ckpt!r} not found")
 
 
+def _check_scope(args, unrecorded=None):
+    """Without --b200_cali_data_out: _require_resume.  With it: the full-precision run that writes calibration data;
+    `unrecorded` names the script's selected sampler option when that sampler's steps are not recorded."""
+    if not _cali_out(args):
+        return _require_resume(args)
+    if args.ptq:
+        raise SystemExit("--b200_cali_data_out samples the full-precision model (the calibration set comes from its own "
+                         "denoising run): drop --ptq")
+    if unrecorded:
+        raise SystemExit(f"--b200_cali_data_out: {unrecorded} records no calibration entries (the DDIM and PLMS loops do)")
+
+
 def _calibrates(args):
     """--ptq without --resume / --resume_w / --quant_act: weight calibration on the engine, which is all the reference
     computes for the weights with --cali_iters 0.  Reconstruction iterations are refused."""
@@ -268,12 +301,25 @@ def _wrap(model, args, a_sym, device, scale_method='max', out_dir="."):
     return qnn
 
 
+def _full_precision(model, args):
+    """QuantModel over `model` in set_quant_state(False, False), no quantizer initialised: the fp32 weights run as
+    bfloat16 planes (graph.WeightOnlyBuilder), the model the reference samples its calibration data with."""
+    import qdiff_b200 as qd
+    wq = {'n_bits': args.weight_bit, 'channel_wise': True, 'scale_method': 'max'}
+    aq = {'n_bits': args.act_bit, 'symmetric': False, 'channel_wise': False, 'scale_method': 'max', 'leaf_param': False}
+    qnn = qd.QuantModel(model=model, weight_quant_params=wq, act_quant_params=aq, sm_abit=args.sm_abit)
+    qnn.set_quant_state(False, False)
+    return qnn
+
+
 def _synthetic(args, expect_family):
     from . import synth
     name = args.b200_synthetic
     if name not in synth.SPECS or synth.SPECS[name]["family"] != expect_family:
         raise SystemExit(f"--b200_synthetic {name!r}: expected one of "
                          f"{[k for k, v in synth.SPECS.items() if v['family'] == expect_family]}")
+    if _cali_out(args):
+        return _full_precision(synth.build_model(name), args), synth.SPECS[name]
     qnn, _ = synth.build_qnn(name)
     return qnn, synth.SPECS[name]
 
@@ -367,8 +413,8 @@ def run_ddim(args):
     per step from the round's seed and keep this rank's slice (dist.step_noise_fn)."""
     import numpy as np
     import torch
-    from . import dist as qdist, samplers, unet
-    _require_resume(args)
+    from . import cali_data, dist as qdist, samplers, unet
+    _check_scope(args, f"--sample_type {args.sample_type}" if args.sample_type != "generalized" else None)
     rank, world, dev = _setup(args.seed)
     if args.cond:
         raise SystemExit("--cond is not valid for the DDIM (CIFAR) script (the reference asserts the same)")
@@ -388,20 +434,13 @@ def run_ddim(args):
                                             in_channels=m["in_channels"], image_size=size,
                                             resamp_with_conv=m.get("resamp_with_conv", True), split_shortcut=args.split,
                                             num_diffusion_timesteps=d["num_diffusion_timesteps"]))
-        if _calibrates(args):
-            # sample_diffusion_ddim.py:113-121: ddim/functions/ckpt_util.get_ckpt_path("ema_<dataset>"), never downloaded
-            data = cfg["data"]
-            name = "cifar10" if data.get("dataset") == "CIFAR10" else f"lsun_{data.get('category')}".replace(
-                "church_outdoor", "church")
-            sub = {"cifar10": "ema_diffusion_cifar10_model/model-790000.ckpt",
-                   "lsun_bedroom": "ema_diffusion_lsun_bedroom_model/model-2388000.ckpt",
-                   "lsun_cat": "ema_diffusion_lsun_cat_model/model-1761000.ckpt",
-                   "lsun_church": "ema_diffusion_lsun_church_model/model-4432000.ckpt"}.get(name)
-            if sub is None:
-                raise SystemExit(f"no pretrained DDIM checkpoint is defined for dataset {name!r}")
-            cache = os.environ.get("XDG_CACHE_HOME", os.path.expanduser("~/.cache"))
-            model.load_state_dict(_base_state(os.path.join(cache, "diffusion_models_converted", sub), "DDIM"), strict=True)
-        qnn = _wrap(model, args, args.a_sym, dev, 'max', args.logdir if args.logdir != "none" else ".")
+        if _cali_out(args):
+            _load_ddim_base(model, cfg)
+            qnn = _full_precision(model, args)
+        else:
+            if _calibrates(args):
+                _load_ddim_base(model, cfg)
+            qnn = _wrap(model, args, args.a_sym, dev, 'max', args.logdir if args.logdir != "none" else ".")
         batch = cfg["sampling"]["batch_size"]
     if d.get("beta_schedule", "linear") != "linear":
         raise SystemExit("only the linear beta schedule of the reference's configs is supported")
@@ -421,6 +460,7 @@ def run_ddim(args):
     per = _shard(batch, world)
     n_rounds = max(1, -(-args.max_images // batch))
     model = _CountingModel(lambda xx, tt: qnn(xx, tt))
+    cali = cali_data.CaliData(rank, world) if _cali_out(args) else None
     outs, t0 = [], time.time()
     for r in range(n_rounds):
         (x,) = qdist.shard_like_single_process((batch, ch, size, size), args.seed + r, rank, world)
@@ -429,8 +469,12 @@ def run_ddim(args):
         if kind == "generalized":
             noise_gen = torch.Generator().manual_seed(noise_seed)
             full_noise = [torch.randn(batch, ch, size, size, generator=noise_gen) for _ in seq] if args.eta > 0 else None
+            rec = cali_data.StepRecorder(len(seq)) if cali else None
             x = samplers.generalized_steps(x.to(dev), seq, model, betas, eta=args.eta,
-                                           noise_fn=(lambda k, shape, d_: full_noise[k][lo:lo + per].to(d_)) if full_noise else None)
+                                           noise_fn=(lambda k, shape, d_: full_noise[k][lo:lo + per].to(d_)) if full_noise else None,
+                                           record=rec)
+            if cali:
+                cali.add(rec)
         elif kind == "ddpm_noisy":
             x = samplers.ddpm_steps(x.to(dev), seq, model, betas,
                                     noise_fn=qdist.step_noise_fn((batch, ch, size, size), noise_seed, rank, world))
@@ -446,7 +490,26 @@ def run_ddim(args):
         print(f"{imgs.shape[0]} images, {kind} sampler, {nfe} UNet calls each, {dt:.2f} s -> {imgs.shape[0] / dt:.2f} "
               f"images/s on {world} GPU(s)")
     meta = dict(kind="images", steps=len(seq) if seq is not None else args.timesteps, sampler=kind, nfe=nfe)
+    if cali:
+        cali.save(_cali_out(args), dict(family="ddim", sampler=kind, steps=len(seq), skip_type=args.skip_type,
+                                                eta=args.eta, scale=1.0, seed=args.seed))
     return _save(args, args.logdir if args.logdir != "none" else ".", imgs, meta, rank)
+
+
+def _load_ddim_base(model, cfg):
+    """sample_diffusion_ddim.py:113-121: the EMA checkpoint ddim/functions/ckpt_util.get_ckpt_path("ema_<dataset>")
+    returns, under $XDG_CACHE_HOME; never downloaded."""
+    data = cfg["data"]
+    name = "cifar10" if data.get("dataset") == "CIFAR10" else f"lsun_{data.get('category')}".replace(
+        "church_outdoor", "church")
+    sub = {"cifar10": "ema_diffusion_cifar10_model/model-790000.ckpt",
+           "lsun_bedroom": "ema_diffusion_lsun_bedroom_model/model-2388000.ckpt",
+           "lsun_cat": "ema_diffusion_lsun_cat_model/model-1761000.ckpt",
+           "lsun_church": "ema_diffusion_lsun_church_model/model-4432000.ckpt"}.get(name)
+    if sub is None:
+        raise SystemExit(f"no pretrained DDIM checkpoint is defined for dataset {name!r}")
+    cache = os.environ.get("XDG_CACHE_HOME", os.path.expanduser("~/.cache"))
+    model.load_state_dict(_base_state(os.path.join(cache, "diffusion_models_converted", sub), "DDIM"), strict=True)
 
 
 # ---------------------------------------------------------------------------------------------- sample_diffusion_ldm
@@ -468,8 +531,8 @@ def run_ldm(args):
     --dpm DPM-Solver++, otherwise DDIM.  Saves the LATENTS; with --b200_decode also the images, decoded by the first
     stage on the engine (qdiff_b200.first_stage)."""
     import torch
-    from . import dist as qdist, samplers, unet
-    _require_resume(args)
+    from . import cali_data, dist as qdist, samplers, unet
+    _check_scope(args, "--dpm" if args.dpm else "-v" if args.vanilla_sample else None)
     rank, world, dev = _setup(args.seed)
     if args.b200_synthetic:
         qnn, spec = _synthetic(args, "ldm")
@@ -479,16 +542,13 @@ def run_ldm(args):
         cfg = _ldm_config(args)["model"]["params"]
         up = dict(cfg["unet_config"]["params"])
         model = unet.UNetModel(**up)
-        if _calibrates(args):
-            # sample_diffusion_ldm.py:384-450: -r names the checkpoint (or its logdir's model.ckpt); EMA weights
-            base = args.resume_base
-            sd = _base_state(base if os.path.isfile(base) else os.path.join(base.rstrip("/"), "model.ckpt"), "-r")
-            ema = {k: sd["model_ema." + ("diffusion_model." + k).replace(".", "")] for k in model.state_dict()
-                   if "model_ema." + ("diffusion_model." + k).replace(".", "") in sd}
-            if len(ema) != len(model.state_dict()):
-                raise SystemExit(f"-r {base!r}: the checkpoint has no EMA copy (model_ema.*) of every UNet parameter")
-            model.load_state_dict(ema, strict=True)
-        qnn = _wrap(model, args, args.a_sym, dev, 'mse', args.logdir if args.logdir != "none" else ".")
+        if _cali_out(args):
+            _load_ldm_base(model, args.resume_base)
+            qnn = _full_precision(model, args)
+        else:
+            if _calibrates(args):
+                _load_ldm_base(model, args.resume_base)
+            qnn = _wrap(model, args, args.a_sym, dev, 'mse', args.logdir if args.logdir != "none" else ".")
         ch, size = cfg["channels"], cfg["image_size"]
         sched = dict(timesteps=cfg.get("timesteps", 1000), linear_start=cfg.get("linear_start", 1e-4),
                      linear_end=cfg.get("linear_end", 2e-2))
@@ -501,6 +561,7 @@ def run_ldm(args):
     else:
         sampler, kind = samplers.DDIMSampler(model, schedule), "ddim"
     per = _shard(args.batch_size, world)
+    cali = cali_data.CaliData(rank, world) if _cali_out(args) else None
     outs, t0, r = [], time.time(), 0
     while sum(o.shape[0] for o in outs) < args.n_samples:
         (x_T,) = qdist.shard_like_single_process((args.batch_size, ch, size, size), args.seed + r, rank, world)
@@ -516,8 +577,12 @@ def run_ldm(args):
         elif args.dpm:    # convsample_dpm (sample_diffusion_ldm.py:96-103): deterministic, eta is not used
             z, _ = sampler.sample(S=args.custom_steps, batch_size=per, shape=(ch, size, size), x_T=x_T)
         else:
+            rec = cali_data.StepRecorder(len(samplers.make_ddim_timesteps("uniform", args.custom_steps,
+                                                                         schedule.num_timesteps))) if cali else None
             z, _ = sampler.sample(S=args.custom_steps, batch_size=per, shape=(ch, size, size), eta=args.eta, x_T=x_T,
-                                  noise_fn=noise_fn)
+                                  noise_fn=noise_fn, record=rec)
+            if cali:
+                cali.add(rec)
         outs.append(qdist.gather_latents(z, world))
         r += 1
     z = torch.cat(outs)[:args.n_samples]
@@ -528,6 +593,9 @@ def run_ldm(args):
         print(f"{z.shape[0]} latents, {kind} sampler, {nfe} UNet calls each, {dt:.2f} s -> {z.shape[0] / dt:.2f} /s on "
               f"{world} GPU(s)")
     meta = dict(kind="latents", steps=nfe if args.vanilla_sample else args.custom_steps, eta=args.eta, sampler=kind, nfe=nfe)
+    if cali:
+        cali.save(_cali_out(args), dict(family="ldm", sampler=kind, steps=args.custom_steps, eta=args.eta,
+                                                scale=1.0, seed=args.seed))
     if args.b200_decode and rank == 0:
         fs, sf = _first_stage(args, args.b200_synthetic, None if args.b200_synthetic else cfg, dev)
         t1 = time.time()
@@ -535,6 +603,16 @@ def run_ldm(args):
         torch.cuda.synchronize()
         print(f"decoded {tuple(meta['images'].shape)} in {time.time() - t1:.2f} s (first stage on the engine, precision {args.b200_decode_precision})")
     return _save(args, args.logdir if args.logdir != "none" else ".", z, meta, rank)
+
+
+def _load_ldm_base(model, base):
+    """sample_diffusion_ldm.py:384-450: -r names the checkpoint (or its logdir's model.ckpt); EMA weights."""
+    sd = _base_state(base if os.path.isfile(base) else os.path.join(base.rstrip("/"), "model.ckpt"), "-r")
+    ema = {k: sd["model_ema." + ("diffusion_model." + k).replace(".", "")] for k in model.state_dict()
+           if "model_ema." + ("diffusion_model." + k).replace(".", "") in sd}
+    if len(ema) != len(model.state_dict()):
+        raise SystemExit(f"-r {base!r}: the checkpoint has no EMA copy (model_ema.*) of every UNet parameter")
+    model.load_state_dict(ema, strict=True)
 
 
 # ---------------------------------------------------------------------------------------------- txt2img
@@ -590,8 +668,8 @@ def run_txt2img(args):
     get_learned_conditioning per batch; batch j of iteration n starts from seed + 1 + n * batches + j), else a seeded
     N(0,1) context.  Saves the latents, with --b200_decode also the decoded images."""
     import torch
-    from . import dist as qdist, samplers, unet
-    _require_resume(args)
+    from . import cali_data, dist as qdist, samplers, unet
+    _check_scope(args)
     if not args.cond:
         raise SystemExit("txt2img needs --cond (the reference asserts the same)")
     enc_sd = _text_encoder_state(args)
@@ -608,12 +686,13 @@ def run_txt2img(args):
         cfg = _load_yaml(args.config)["model"]["params"]
         model = unet.UNetModel(**dict(cfg["unet_config"]["params"]))
         model.split = bool(args.split)
-        if _calibrates(args):
-            # txt2img.py:57-66, 358: the UNet of --ckpt, keys model.diffusion_model.*
-            sd = _base_state(args.ckpt, "--ckpt")
-            pre = "model.diffusion_model."
-            model.load_state_dict({k[len(pre):]: v for k, v in sd.items() if k.startswith(pre)}, strict=True)
-        qnn = _wrap(model, args, False, dev, 'mse', args.outdir)
+        if _cali_out(args):
+            _load_sd_base(model, args.ckpt)
+            qnn = _full_precision(model, args)
+        else:
+            if _calibrates(args):
+                _load_sd_base(model, args.ckpt)
+            qnn = _wrap(model, args, False, dev, 'mse', args.outdir)
         sched = dict(timesteps=cfg.get("timesteps", 1000), linear_start=cfg["linear_start"], linear_end=cfg["linear_end"])
         ctx_shape = (77, cfg["unet_config"]["params"]["context_dim"])
     Sampler = samplers.PLMSSampler if args.plms else samplers.DDIMSampler
@@ -642,23 +721,33 @@ def run_txt2img(args):
             if uc_full is None:
                 raise SystemExit("--scale != 1 needs the empty-prompt embedding 'uc' in --b200_context")
             uc = uc_full.float().expand(B, -1, -1)[lo:lo + per].contiguous().to(dev)
+        if _cali_out(args) and uc_full is None:
+            raise SystemExit("--b200_cali_data_out needs the empty-prompt embedding 'uc' in --b200_context (the file's ucs)")
+        c_all, uc_all = c_full, uc_full
     shape = (args.C, args.H // args.f, args.W // args.f)
     start = None
     if args.fixed_code:
         (start,) = qdist.shard_like_single_process((B,) + shape, args.seed, rank, world)
+    cali = cali_data.CaliData(rank, world) if _cali_out(args) else None
     outs, prompts_all, t0 = [], [], time.time()
     for n in range(args.n_iter):
         for j, prompts in enumerate(batches):
             if encoder is not None:     # every rank encodes the whole batch and keeps its slice (as with the noise)
-                uc = encoder.encode(B * [""])[lo:lo + per].contiguous() if args.scale != 1.0 else None
-                c = encoder.encode(list(prompts))[lo:lo + per].contiguous()
+                uc_all = encoder.encode(B * [""]) if args.scale != 1.0 or cali else None
+                c_all = encoder.encode(list(prompts))
+                uc = uc_all[lo:lo + per].contiguous() if args.scale != 1.0 else None
+                c = c_all[lo:lo + per].contiguous()
                 prompts_all += list(prompts)
             x_T = start
             if x_T is None:
                 (x_T,) = qdist.shard_like_single_process((B,) + shape, args.seed + 1 + n * len(batches) + j, rank, world)
+            rec = cali_data.StepRecorder(len(samplers.make_ddim_timesteps("uniform", args.ddim_steps,
+                                                                         sampler.ddpm_num_timesteps))) if cali else None
             z, _ = sampler.sample(S=args.ddim_steps, conditioning=c, batch_size=per, shape=shape, verbose=False,
                                   unconditional_guidance_scale=args.scale, unconditional_conditioning=uc, eta=args.ddim_eta,
-                                  x_T=x_T)
+                                  x_T=x_T, record=rec)
+            if cali:
+                cali.add(rec, c_all, uc_all)
             outs.append(qdist.gather_latents(z, world))
     z = torch.cat(outs)
     torch.cuda.synchronize()
@@ -669,6 +758,10 @@ def run_txt2img(args):
     meta = dict(kind="latents", steps=args.ddim_steps, scale=args.scale, prompt=args.prompt)
     if encoder is not None:
         meta["prompts"] = prompts_all           # the prompt of every image, in sample order
+    if cali:
+        cali.save(_cali_out(args), dict(family="sd", sampler="plms" if args.plms else "ddim", steps=args.ddim_steps,
+                                                eta=args.ddim_eta, scale=args.scale, seed=args.seed,
+                                                **({"prompts": prompts_all} if encoder is not None else {})))
     if args.b200_decode and rank == 0:
         fs, sf = _first_stage(args, args.b200_synthetic, None if args.b200_synthetic else cfg, dev)
         t1 = time.time()
@@ -676,3 +769,10 @@ def run_txt2img(args):
         torch.cuda.synchronize()
         print(f"decoded {tuple(meta['images'].shape)} in {time.time() - t1:.2f} s (first stage on the engine, precision {args.b200_decode_precision})")
     return _save(args, args.outdir, z, meta, rank)
+
+
+def _load_sd_base(model, ckpt):
+    """txt2img.py:57-66, 358: the UNet of --ckpt, keys model.diffusion_model.*"""
+    sd = _base_state(ckpt, "--ckpt")
+    pre = "model.diffusion_model."
+    model.load_state_dict({k[len(pre):]: v for k, v in sd.items() if k.startswith(pre)}, strict=True)

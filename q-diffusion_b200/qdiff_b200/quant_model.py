@@ -4,7 +4,8 @@ Quantisation states the engine realises (set_quant_state, reference :52-55):
     (True, True)   weights and activations quantised (W4A8 / W8A8): INT8 wgmma GEMMs, all four UNet configurations;
     (True, False)  weight-only (what resume_cali_model(..., quant_act=False) leaves, qdiff/utils.py:407): fp32 activations
                    as bfloat16 x3 planes against exact bfloat16 weight codes, fp32 accumulation; DDIM (CIFAR) family;
-    (False, False) full precision: NOT realised (it is the reference's own path for FP baselines / calibration data).
+    (False, False) full precision (the reference's path for FP baselines and calibration data): fp32 activations and
+                   weights as bfloat16 x3 planes, fp32 accumulation (graph.WeightOnlyBuilder; qdiff_b200.cali_data).
 Activation quantizers must be per-tensor and at most 8 bits (16 for the softmax quantizer); graph.Builder.qp refuses
 anything else instead of wrapping codes.
 

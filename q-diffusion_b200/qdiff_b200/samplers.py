@@ -141,7 +141,8 @@ class _LatentSampler:
 class DDIMSampler(_LatentSampler):
     @torch.no_grad()
     def sample(self, S, batch_size, shape, conditioning=None, eta=0., x_T=None, unconditional_guidance_scale=1.,
-               unconditional_conditioning=None, noise_fn=None, verbose=False, **kwargs):
+               unconditional_conditioning=None, noise_fn=None, verbose=False, record=None, **kwargs):
+        """record(i, x, t), when given, is called before step i's UNet call with that call's un-doubled input."""
         self.make_schedule(S, ddim_eta=eta)
         dev = torch.device("cuda", torch.cuda.current_device())
         size = (batch_size,) + tuple(shape)
@@ -152,6 +153,8 @@ class DDIMSampler(_LatentSampler):
         for i, step in enumerate(time_range):
             index = total - i - 1
             ts = torch.full((batch_size,), int(step), device=dev, dtype=torch.long)
+            if record is not None:
+                record(i, img, ts)
             eps, s = self._model_eps(img, ts, conditioning, unconditional_conditioning, unconditional_guidance_scale)
             sigma = float(self.ddim_sigmas[index])
             noise = None
@@ -168,7 +171,9 @@ class PLMSSampler(_LatentSampler):
 
     @torch.no_grad()
     def sample(self, S, batch_size, shape, conditioning=None, eta=0., x_T=None, unconditional_guidance_scale=1.,
-               unconditional_conditioning=None, verbose=False, **kwargs):
+               unconditional_conditioning=None, verbose=False, record=None, **kwargs):
+        """record(i, x, t), when given, is called before step i's first UNet call (not the provisional second call of
+        step 0) with that call's un-doubled input."""
         if eta != 0:
             raise ValueError('ddim_eta must be 0 for PLMS')
         self.make_schedule(S, ddim_eta=0.)
@@ -185,6 +190,8 @@ class PLMSSampler(_LatentSampler):
             ts = torch.full((batch_size,), int(step), device=dev, dtype=torch.long)
             kw = dict(a_t=self.ddim_alphas[index], a_prev=self.ddim_alphas_prev[index], sigma=0.0,
                       sqrt_one_minus_at=self.ddim_sqrt_one_minus_alphas[index])
+            if record is not None:
+                record(i, img, ts)
             eps, s = self._model_eps(img, ts, conditioning, uc, sc)
             e_t = torch.empty_like(img)
             if len(old_eps) == 0:
@@ -292,9 +299,10 @@ class DPMSolverSampler(_LatentSampler):
 
 
 @torch.no_grad()
-def generalized_steps(x, seq, model, b, eta=0.0, noise_fn=None):
+def generalized_steps(x, seq, model, b, eta=0.0, noise_fn=None, record=None):
     """DDIM loop of the CIFAR script (ddim/functions/denoising.py:10-32).  x: [n,C,H,W] on CUDA, seq: list of
-    timesteps, b: betas (1-D tensor).  Returns the final x only (device resident; no per-step host copies)."""
+    timesteps, b: betas (1-D tensor).  Returns the final x only (device resident; no per-step host copies).
+    record(k, x, t), when given, is called before step k's UNet call with that call's input."""
     n = x.size(0)
     dev = x.device
     beta = torch.cat([torch.zeros(1), b.detach().cpu().float()], dim=0)
@@ -305,6 +313,8 @@ def generalized_steps(x, seq, model, b, eta=0.0, noise_fn=None):
     for k, (i, j) in enumerate(zip(reversed(seq), reversed(seq_next))):
         t = (torch.ones(n) * i).to(dev)
         at, at_next = float(acp[int(i) + 1]), float(acp[int(j) + 1])
+        if record is not None:
+            record(k, cur, t)
         et = model(cur, t)
         c1 = eta * math.sqrt((1 - at / at_next) * (1 - at_next) / (1 - at))
         noise = None

@@ -14,4 +14,4 @@ for p in (ROOT, os.path.join(ROOT, "q-diffusion_b200")):
 from qdiff_b200 import cli  # noqa: E402
 
 if __name__ == "__main__":
-    cli.run_ddim(cli.ddim_parser().parse_args())
+    cli.run_ddim(cli.script_parser(cli.ddim_parser()).parse_args())
