@@ -10,6 +10,7 @@ Reference graph being lowered:
   Model.forward      ddim/models/diffusion.py:308-360
 with the Quant*Block forwards of qdiff/quant_block.py (cited at each lowering function).
 """
+import copy
 import ctypes as C
 import math
 import os
@@ -41,6 +42,16 @@ class Act:
         """The [rows, cols] tensor this Act denotes (a strided view when it lives inside a wider buffer)."""
         t = self.t if self.t.dim() == 2 else self.t.view(-1, self.ld)      # transposed V^T codes are allocated flat
         return t[:self.rows, self.col0:self.col0 + self.cols]
+
+
+def _frozen(v):
+    """A spec value with every Act in it copied: cfg_split widens the prefix's Acts to both halves after their ops were
+    recorded, and a spec describes the rows its op touches when it runs."""
+    if isinstance(v, Act):
+        return copy.copy(v)
+    if isinstance(v, (tuple, list)):
+        return type(v)(_frozen(x) for x in v)
+    return v
 
 
 def _qt(qp):
@@ -209,14 +220,16 @@ class Builder:
                 continue
             seen.add(id(a))
             half = a.rows
+            first = Act(a.t, half, a.cols, ld=a.ld, col0=a.col0)           # the rows of the first half (spec only)
             self.misc(_lib.QD_OP_COPY2D, a.ptr, a.ptr + 4 * half * a.ld, half, a.cols, ld_src=a.ld, ld_dst=a.ld,
-                      label="cfg.dup", spec=dict(kind="cfg_dup"))
+                      label="cfg.dup",
+                      spec=dict(kind="cfg_dup", src=first, dst=Act(a.t[half:], half, a.cols, ld=a.ld, col0=a.col0)))
             ent = self.gn_slabs.get(id(a.t))
             if ent is not None and half % 32 == 0 and self._covered(ent[1], a.col0, a.col0 + a.cols):
                 ld2 = 2 * ent[0].shape[1]
                 src = ent[0].data_ptr() + 8 * a.col0
                 self.misc(_lib.QD_OP_COPY2D, src, src + 4 * (half // 32) * ld2, half // 32, 2 * a.cols, ld_src=ld2, ld_dst=ld2,
-                          label="cfg.dup.slabs", spec=dict(kind="cfg_dup"))
+                          label="cfg.dup.slabs", spec=dict(kind="cfg_dup", src=first, slabs=ent[0]))
             a.rows = 2 * half
         for a in self._prefix_acts:          # buffers allocated for both halves: the Act now spans both
             if id(a) not in seen:
@@ -232,6 +245,8 @@ class Builder:
         """Record one engine op.  `spec` describes the op's operands and semantics in host terms (Acts, quantizer
         tuples, folded weights): the in-situ parity tests replay the program op by op and check every op against the
         CPU oracle on the engine's own inputs (tests/test_insitu_gpu.py).  Pure metadata, never read on the hot path."""
+        if self.prefix and spec is not None:
+            spec = {k: _frozen(v) for k, v in spec.items()}
         self._pending.append((kind, desc, label, flops, spec if spec is not None else {"kind": "unspecified"},
                               self._static_depth > 0 and self.hoist_ctx))
 

@@ -39,7 +39,7 @@ def rd_f32(act):
 
 
 def rd_codes(act):
-    t = act.logical().detach().cpu()
+    t = act.logical().detach().to(DEV)
     if getattr(act, "f16", False):         # attention Q/K operands as fp16 (code - zero_point): back to codes
         return t.to(torch.float64).round().to(torch.int64) + int(act.zp[0])
     return t.to(torch.int64)               # uint8 -> 0..255, int8 -> -128..127
@@ -53,10 +53,12 @@ def vt_positions(T):
 
 def quant(y, q):
     """UniformAffineQuantizer codes (quant_layer.py:82-87) of a double tensor; q = (delta, zp, lo, hi).
-    The division is carried out in fp32 like the reference (y is fp32-representable or is rounded to fp32 first)."""
+    The division is carried out in fp32 like the reference (y is fp32-representable or is rounded to fp32 first).  The
+    divisor lives on y's device: torch divides a CUDA tensor by a CPU scalar as a product with its fp32 reciprocal, which
+    is one code off at about one position in a million."""
     delta, zp, lo, hi = q
     yf = y.to(torch.float32)
-    return torch.clamp(torch.round(yf / torch.tensor(delta, dtype=torch.float32)) + zp, lo, hi).to(torch.int64)
+    return torch.clamp(torch.round(yf / torch.tensor(delta, dtype=torch.float32, device=yf.device)) + zp, lo, hi).to(torch.int64)
 
 
 class Report:
@@ -112,7 +114,8 @@ def _cmp_f32(rep, idx, label, kind, got, ref, tol, what="fp32"):
 _INPUTS = {"split3": ["src"], "gemm_wo": ["rowvec", "residual"], "attention_fp": ["q", "k", "v"],
            "quantize": ["src"], "groupnorm": ["x"], "layernorm": ["x"], "gemm": ["a", "rowvec", "residual"],
            "attention": ["q", "k", "vt"], "im2col": ["src"], "copy2d": ["src"], "upsample2x": ["src"],
-           "avgpool2x": ["src"], "nhwc_to_nchw": ["src"], "gemm_fp": ["rowvec", "residual"], "vq_lookup": ["src"]}
+           "avgpool2x": ["src"], "nhwc_to_nchw": ["src"], "gemm_fp": ["rowvec", "residual"], "vq_lookup": ["src"],
+           "cfg_dup": ["src"]}
 
 
 def snapshot(spec):
@@ -140,6 +143,9 @@ def snapshot(spec):
         pre["t"] = spec["t"].detach().to(DEV, torch.float32)
     if spec["kind"] == "nchw_to_nhwc":
         pre["src"] = spec["src"].detach().to(DEV, torch.float64)
+    if spec["kind"] == "cfg_dup" and "slabs" in spec:
+        a = spec["src"]
+        pre["slabs"] = spec["slabs"].detach()[:a.rows // 32, a.col0:a.col0 + a.cols].to(DEV, torch.float64)
     return pre
 
 
@@ -233,9 +239,9 @@ def check_im2col(rep, i, label, s, pre):
     pc = s["pad_code"]
     if s["src"].signed:
         pc = pc - 256 if pc > 127 else pc
-    xp = torch.full((B, H + 3, W + 3, C), pc, dtype=torch.int64)
+    xp = torch.full((B, H + 3, W + 3, C), pc, dtype=torch.int64, device=src.device)
     xp[:, pt:pt + H, pl:pl + W] = x
-    ref = torch.zeros(B, Ho, Wo, s["k_to"], dtype=torch.int64)
+    ref = torch.zeros(B, Ho, Wo, s["k_to"], dtype=torch.int64, device=src.device)
     st = s["stride"]
     for ky in range(3):
         for kx in range(3):
@@ -245,7 +251,7 @@ def check_im2col(rep, i, label, s, pre):
 
 def check_gemm(rep, i, label, s, pre):
     N, taps, Cred = s["N"], s["taps"], s["C"]
-    ws = s["ws"].double()
+    ws = s["ws"].to(DEV, torch.float64)
     a = pre["a"][:, s["a_cols"]:s["a_cols"] + (Cred if taps == 1 else Cred)]
     zx = s["zx"]
     M = a.shape[0]
@@ -261,15 +267,15 @@ def check_gemm(rep, i, label, s, pre):
         if w2.shape[1] < Cred:
             w2 = F.pad(w2, (0, Cred - w2.shape[1]))
         acc = (a.double() - zx) @ w2.t()
-    t_main = acc * s["scale"].double()[None, :]
+    t_main = acc * s["scale"].to(DEV, torch.float64)[None, :]
     y = t_main.clone()
     mag = t_main.abs()
     if s["bias"] is not None:
-        y += s["bias"].double()[None, :]
-        mag += s["bias"].double().abs()[None, :]
+        y += s["bias"].to(DEV, torch.float64)[None, :]
+        mag += s["bias"].to(DEV, torch.float64).abs()[None, :]
     if s["rowvec"] is not None:
         rv = pre["rowvec"][:, :N]
-        img = torch.arange(M) // s["rows_per_batch"]
+        img = torch.arange(M, device=DEV) // s["rows_per_batch"]
         y += rv[img]
         mag += rv[img].abs()
     if s["residual"] is not None:
@@ -283,7 +289,7 @@ def check_gemm(rep, i, label, s, pre):
     if s["out_q"] is not None:
         q = s["oq"]
         if s["geglu"]:
-            r = torch.arange(N)
+            r = torch.arange(N, device=DEV)
             xs, gs = y[:, (r % 8) < 4], y[:, (r % 8) >= 4]
             ref = quant((xs.to(torch.float32) * F.gelu(gs.to(torch.float32))).double(), q)
             got = rd_codes(s["out_q"])
@@ -292,12 +298,12 @@ def check_gemm(rep, i, label, s, pre):
             Bn = M // T
             ref = quant(y, q).reshape(Bn, T, N).permute(0, 2, 1)                 # [B, N, T]
             raw = rd_codes(s["out_q"]).reshape(Bn, N, -1)
-            got = raw[:, :, vt_positions(T)]
+            got = raw[:, :, vt_positions(T).to(DEV)]
         elif s["out_q_head"] is not None:
             d, P = s["out_q_head"]
             ref = quant(y, q)
             raw = rd_codes(s["out_q"])
-            n = torch.arange(N)
+            n = torch.arange(N, device=DEV)
             got = raw[:, (n // d) * P + n % d]
         else:
             ref = quant(y, q)
@@ -308,8 +314,8 @@ def check_gemm(rep, i, label, s, pre):
 def check_attention(rep, i, label, s, pre):
     B, heads, d, Tq, Tk = s["B"], s["heads"], s["d"], s["Tq"], s["Tk"]
     qa, ka, va = s["q"], s["k"], s["vt"]
-    h = torch.arange(heads)[:, None]
-    c = torch.arange(d)[None, :]
+    h = torch.arange(heads, device=DEV)[:, None]
+    c = torch.arange(d, device=DEV)[None, :]
     qcols = (s["q_layout"][0] + h * s["q_layout"][1] + c).reshape(-1)
     kcols = (s["k_layout"][0] + h * s["k_layout"][1] + c).reshape(-1)
     qf = (pre["q"][:, qcols].double() - qa.zp[0]) * float(qa.delta[0])
@@ -317,14 +323,21 @@ def check_attention(rep, i, label, s, pre):
     qf = qf.reshape(B, Tq, heads, d).permute(0, 2, 1, 3)
     kf = kf.reshape(B, Tk, heads, d).permute(0, 2, 1, 3)
     vrows = (s["v_layout"][0] + h * s["v_layout"][1] + c).reshape(-1)
-    vt = pre["vt"].reshape(B, -1, pre["vt"].shape[1])[:, vrows][:, :, vt_positions(Tk)]      # [B, heads*d, Tk]
+    vt = pre["vt"].reshape(B, -1, pre["vt"].shape[1])[:, vrows][:, :, vt_positions(Tk).to(DEV)]      # [B, heads*d, Tk]
     vf = ((vt.double() - va.zp[0]) * float(va.delta[0])).reshape(B, heads, d, Tk).permute(0, 1, 3, 2)
-    # scores: exact integers x (delta_q*delta_k*extra) like the engine and, up to fp32 rounding, like the reference
-    sim = torch.einsum("bhid,bhjd->bhij", qf, kf) * s["scale_extra"]
-    p = torch.softmax(sim.to(torch.float32), dim=-1)                # the reference's softmax runs in fp32
     dw, zw, lo, hi = s["qw"]
-    pc = torch.clamp(torch.round(p / torch.tensor(dw, dtype=torch.float32)) + zw, lo, hi).double()
-    out = torch.einsum("bhij,bhjd->bhid", (pc - zw) * dw, vf)
+    out = torch.empty(B, heads, Tq, d, dtype=torch.float64, device=qf.device)
+    hc = max(1, min(heads, (1 << 26) // (Tq * Tk)))      # heads per chunk: the float64 scores of SD's T = 9216 are 680 MB a head
+    for b in range(B):
+        for h0 in range(0, heads, hc):
+            hs = slice(h0, h0 + hc)
+            # scores: exact integers x (delta_q*delta_k*extra) like the engine and, up to fp32 rounding, like the reference
+            sim = torch.einsum("hid,hjd->hij", qf[b, hs], kf[b, hs]) * s["scale_extra"]
+            p = torch.softmax(sim.to(torch.float32), dim=-1)                # the reference's softmax runs in fp32
+            del sim
+            pc = torch.clamp(torch.round(p / torch.tensor(dw, dtype=torch.float32, device=p.device)) + zw, lo, hi).double()
+            del p
+            out[b, hs] = torch.einsum("hij,hjd->hid", (pc - zw) * dw, vf[b, hs])
     ref = out.permute(0, 2, 1, 3).reshape(B * Tq, heads * d)
     if s["oq"] is None:
         got = rd_f32(s["out"])
@@ -362,6 +375,27 @@ def check_misc(rep, i, label, s, pre):
         ref = x.reshape(x.shape[0], x.shape[1], -1).permute(0, 2, 1).reshape(-1, x.shape[1])
         got = rd_f32(s["dst"])
         rep.add(i, label, k, "fp32=", ref.numel(), int((got != ref).sum()), float((got - ref).abs().max()), bool(torch.equal(got, ref)))
+    elif k == "cfg_dup" and "slabs" not in s:
+        # guidance prefix: the second half of the doubled batch is a copy of the first, bit for bit
+        got, ref = rd_f32(s["dst"]), pre["src"]
+        rep.add(i, label, k, "fp32=", ref.numel(), int((got != ref).sum()), float((got - ref).abs().max()), bool(torch.equal(got, ref)))
+    elif k == "cfg_dup":
+        # ... and the GroupNorm slab sums of the first half (32-row sums of x and x^2 per column, left by the GEMM that
+        # wrote it) copied for the second: bit for bit, and equal to float64 sums of the copied rows within the GEMM
+        # statistics bound of test_gemm_matrix_gpu.py (check_gn)
+        n, a = pre["src"].shape[0] // 32, s["src"]
+        got = s["slabs"].detach()[n:2 * n, a.col0:a.col0 + a.cols].to(DEV, torch.float64)
+        ref = pre["slabs"]
+        rep.add(i, label, k, "slabs=", ref.numel(), int((got != ref).sum()), float((got - ref).abs().max()), bool(torch.equal(got, ref)))
+        x = pre["src"].reshape(n, 32, -1)
+        bad = 0
+        worst = 0.0
+        for j, want in enumerate((x.sum(dim=1), (x * x).sum(dim=1))):
+            tol = 1e-5 * max(1.0, float(want.abs().max()))
+            err = (got[..., j] - want).abs()
+            bad += int((err > tol).sum())
+            worst = max(worst, float(err.max()) / tol)
+        rep.add(i, label, k, "slabs~", got.numel(), bad, worst, bad == 0, note="(max err / tol)")
     elif k == "nhwc_to_nchw":
         dst = s["dst"].detach().to(DEV, torch.float64)
         B, C = dst.shape[0], dst.shape[1]
@@ -670,7 +704,7 @@ CHECKS = {"split3": check_split3, "im2col_bytes": check_im2col_bytes, "gemm_wo":
           "quantize": check_quantize, "groupnorm": check_groupnorm, "layernorm": check_layernorm, "im2col": check_im2col,
           "gemm": check_gemm, "attention": check_attention, "gemm_fp": check_gemm_fp, "plane_tile": check_plane_tile,
           "softmax_rows": check_softmax_rows, "vq_lookup": check_vq_lookup, "embed": check_embed}
-MISC_KINDS = ("copy2d", "upsample2x", "avgpool2x", "timestep_emb", "nchw_to_nhwc", "nhwc_to_nchw")      # check_misc
+MISC_KINDS = ("copy2d", "upsample2x", "avgpool2x", "timestep_emb", "nchw_to_nhwc", "nhwc_to_nchw", "cfg_dup")  # check_misc
 MARKER = "gemm_fp_pass"     # the later launches of a gemm_fp logical op: checked as part of it, never on their own
 
 

@@ -30,10 +30,10 @@ def _dump(name, rep, extra=None):
         pass
 
 
-def _run(name, qnn, x, t, ctx, cuda):
+def _run(name, qnn, x, t, ctx, cuda, device="cpu"):
     c = ctx.to(cuda) if ctx is not None else None
     prog = qnn.program(x.to(cuda), c)
-    rep = insitu.verify_program(prog, x, t, ctx)
+    rep = insitu.verify_program(prog, x, t, ctx, device=device)
     kinds = {s["kind"] for s in prog.op_specs}
     print(f"\n[{name}] in-situ per-op parity: {prog.nops} ops, kinds {sorted(kinds)}\n{rep.summary()}")
     txt = rep.text()
@@ -63,12 +63,13 @@ def test_every_op_matches_oracle_on_golden_unets(cuda, name):
 
 @pytest.mark.parametrize("name,batch", [("cifar10", 2), ("lsun_church", 1), ("sd_v1", 1)])
 def test_every_op_matches_oracle_fullsize(cuda, name, batch):
-    """BASELINE.json UNets at full size (cfg 2 CIFAR-10 W4A8 split, cfg 5 LSUN-church W8A8, cfg 4 SD v1-4 W4A8 sm16)."""
+    """BASELINE.json UNets at full size (cfg 2 CIFAR-10 W4A8 split, cfg 5 LSUN-church W8A8, cfg 4 SD v1-4 W4A8 sm16); the
+    oracle runs on the device."""
     from qdiff_b200 import synth
     qnn, ckpt = synth.build_qnn(name)
     qnn.record_op_specs = True
     x, t, ctx = synth.calib_inputs(name, batch=batch, seed=4242)
-    prog, rep = _run(f"{name}_full", qnn, x, t, ctx, cuda)
+    prog, rep = _run(f"{name}_full", qnn, x, t, ctx, cuda, device=cuda)        # the float64 oracle on the device
     _dump(f"{name}_full", rep, dict(nops=prog.nops))
     fails = rep.failures()
     assert not fails, "\n".join(f"op {r['idx']} {r['kind']} {r['label']} {r['what']} bad={r['nbad']}/{r['n']} max={r['maxdiff']}"
